@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- CTU-analysis throughput (CTUs/s) of the B200 block-primitive path on the BASELINE.json configs.
+"""bench.py -- CTU-analysis throughput (CTUs/s) of the CUDA block-primitive path on the BASELINE.json configs.
 
   --config c3 (default) : 3840x2160  8-bit preset slow    : 4 refs, STAR, merange 57, subme 3, rect, chroma-SATD on (4:2:0)
   --config c4           : 3840x2160 10-bit preset slower  : 5 refs, subme 4, rect + AMP, chroma-SATD on
@@ -67,7 +67,7 @@ def env_int(name, default):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -147,7 +147,24 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
+
+
+DUMP_LIMIT = 64 * 10 ** 6      # bytes of --dump-outputs in all
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: every array as <out_dir>/<name>.npy in float64 (exact for these integer results).  When the set
+    would exceed DUMP_LIMIT, every array keeps the same fraction of its rows, picked by np.random.default_rng(0) and kept in
+    order, so that two runs with the same arguments dump the same rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v) for k, v in arrays.items()}
+    budget = DUMP_LIMIT - 4096 * len(arrays)       # room for the .npy headers
+    frac = min(1.0, budget / float(sum(a.size * 8 for a in arrays.values())))
+    for name, a in arrays.items():
+        if frac < 1.0:
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), int(len(a) * frac), replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------
@@ -264,20 +281,14 @@ def plane_as_tensor(torch, ptr, nbytes, device):
 
 def primitives_leg(lib, reps=3):
     """Per-primitive half of the metric: achieved HBM GB/s of every primitive class at frame scale, 8- and 10-bit
-    (profiles/primitive_bench.py), with the ncu DRAM bytes of the committed capture of the same launches when present."""
+    (profiles/primitive_bench.py)."""
     sys.path.insert(0, os.path.join(ROOT, "profiles"))
     import primitive_bench
-    dram = {}
-    try:
-        for row in json.load(open(os.path.join(ROOT, "profiles", "primitives_r2_ncu.json")))["rows"]:
-            dram[(row["kernel"], row["depth"])] = row.get("dram_bytes")
-    except Exception:
-        pass
     out = []
     for depth in (8, 10):
         for row in primitive_bench.run(lib, depth=depth, reps=reps, frames=24, quiet=True):
             out.append({"kernel": row["kernel"], "depth": depth, "GBps": round(row["GBps"], 1), "frac": round(row["frac_of_measured_peak"], 4),
-                        "algorithmic_bytes": int(row["algorithmic_MB"] * 1e6), "dram_bytes": dram.get((row["kernel"], depth)), "note": row["note"]})
+                        "algorithmic_bytes": int(row["algorithmic_MB"] * 1e6), "note": row["note"]})
     return out
 
 
@@ -547,6 +558,16 @@ def run_ours(args, rank, world, local_rank):
     t_e2e = (time.perf_counter() - t0) * 1000.0
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # what the last e2e step returned for this rank's CTU rows (the whole frame unless the rows are sharded)
+        ranges = [an.row_range(r0, r1) for r0, r1 in my_rows]
+        jobs = np.concatenate([np.arange(j0, j0 + nj) for j0, nj, _, _ in ranges])
+        cus = np.concatenate([np.arange(c0, c0 + nc) for _, _, c0, nc in ranges])
+        mvp = an.me_packed[jobs, 1].view(np.uint32)
+        dump_outputs(args.dump_outputs, {
+            "me_cost": an.me_packed[jobs, 0], "me_mvx": (mvp & 0xffff).astype(np.uint16).view(np.int16),
+            "me_mvy": (mvp >> 16).astype(np.uint16).view(np.int16), "cu_sse": an.cu_sse[cus], "cu_numsig": an.cu_numsig[cus],
+            "cu_ref": an.cu_ref[cus], "intra_cost": an.intra_cost[cus]})
 
     if world > 1:
         t = torch.tensor([t_res, t_e2e], dtype=torch.float64, device=dev)
@@ -582,15 +603,6 @@ def run_ours(args, rank, world, local_rank):
         me_bytes = phase_info[dom][3]
         me_ms = phases[dom]
         achieved = me_bytes / (me_ms / 1000.0) / 1e9
-        traffic = None
-        traffic_src = None
-        try:
-            tr = json.load(open(os.path.join(ROOT, "profiles", "me_r2_traffic.json")))
-            key = "%s_%dx%d_%dbit_%s" % (CFG_NAME, W, H, DEPTH, phase_info[dom][0])
-            if key in tr.get("phases", {}):
-                traffic = float(tr["phases"][key]["dram_bytes_per_step"]); traffic_src = "profiles/me_r2_traffic.json (" + tr.get("how", "ncu") + ")"
-        except Exception:
-            pass
         cfg = workload_config(args.shard)
         sizes = {"resid_bytes": plane * 2 + an.ncoef * 2 + 4 * plane, "intra_bytes": plane + an.ncu * 36 * 4}
         line = {
@@ -603,9 +615,9 @@ def run_ours(args, rank, world, local_rank):
                     "h2d_bytes_per_step": int(an.h2d_bytes(field)) + (W * H // 2 * es if CHROMA else 0), "d2h_bytes_per_step": int(sum(an.d2h_bytes_rows(r0, r1) for r0, r1 in my_rows))},
             "gpu_launches": int(launches),
             "roofline": {"kernel": phase_info[dom][1], "what": phase_info[dom][2], "bound": "hbm", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": int(me_bytes), "kernel_ms": float(me_ms),
-                         "note": "the dominant launches of the step (longest motion-estimation phase); not an HBM-bound kernel family: hundreds of SAD / SATD candidates per job against < 100 B of compulsory traffic, planes L2-resident; the binding resources are the SM's ALU pipe, shared-memory bandwidth and instruction cache (DESIGN.md section 5, profiles/)"},
+                         "note": "the dominant launches of the step (longest motion-estimation phase); not an HBM-bound kernel family: hundreds of SAD / SATD candidates per job against < 100 B of compulsory traffic (the ~70 MB of c3 planes exceed the H100's 50 MB L2, so part of the reads come from HBM); the binding resources are the SM's ALU pipe, shared-memory bandwidth and instruction cache (DESIGN.md section 5)"},
             "phase_rooflines": {pi[0]: {"kernel": pi[1], "ms": float(phases[i]), "algorithmic_bytes": int(pi[3]), "GBps": pi[3] / (phases[i] / 1000.0) / 1e9,
                                         "frac": pi[3] / (phases[i] / 1000.0) / 1e9 / peak} for i, pi in enumerate(phase_info)},
             "stages_ms": {"me_stage": float(stage[0]), "me_prechecks": float(phases[0]), "me_integer_search": float(phases[1]), "me_subpel": float(phases[2]), "residual": float(stage[1]), "intra": float(stage[2])},
@@ -755,6 +767,12 @@ def run_lookahead_ours(args, rank, world, local_rank):
     barrier()
     clocks = sampler.stop()
     costs = {t: la.fr[t[2]]["res"][(t[2] - t[0], t[1] - t[2])]["score"] for t in mine}
+    if args.dump_outputs and rank == 0:
+        # the estimates of the last e2e step, in the order of this rank's (p0, p1, b) triples
+        res = [la.fr[t[2]]["res"][(t[2] - t[0], t[1] - t[2])] for t in mine]
+        dump_outputs(args.dump_outputs, {
+            "triples": np.array(mine), "frame_costs": np.array([[r["score"], r["costEstAq"], r["intraMbs"]] for r in res]),
+            "lowres_costs": np.stack([r["lowresCosts"] for r in res]), "row_satds": np.stack([r["rowSatds"] for r in res])})
     csum = sum(v * (1 + (t[0] * 31 + t[1] * 17 + t[2]) % 13) for t, v in costs.items())
     if world > 1:
         t = torch.tensor([t_res, t_e2e, float(csum)], dtype=torch.float64, device=dev)
@@ -819,7 +837,7 @@ def lookahead_cpu(frames, triples, budget_s=20.0, steps=1):
     kind = "reference" if load_ref(c["depth"]) is not None else "port"
     procs = max(1, min(host_cores(), c["frames"] - 1))
     ncu = ((c["W"] // 2 + 7) // 8) * ((c["H"] // 2 + 7) // 8)
-    # ~0.7 M CUs/s per thread (profiles/lookahead_r1.txt): bound the sample
+    # bound the sample, assuming ~0.5 M CUs/s per host process
     per_triple = ncu / 0.5e6
     maxn = int(max(procs, min(len(triples), budget_s * procs / per_triple)))
     sub = triples[:maxn]
@@ -874,6 +892,8 @@ def main():
     ap.add_argument("--no-chroma", action="store_true", help="luma-only motion estimation (round-1 line; the presets run with the chroma-SATD term)")
     ap.add_argument("--no-pred", action="store_true", help="skip the prediction-cost leg (AMVP / merge / bidir costs) of the N=1 line")
     ap.add_argument("--no-primitives", action="store_true", help="skip the per-primitive HBM GB/s table (8- and 10-bit) of the N=1 line")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the results of the last step as DIR/<name>.npy "
+                                                          "(float64, at most 64 MB in all: a fixed row sample of larger results)")
     args = ap.parse_args()
     global CFG, CFG_NAME
     CFG_NAME = args.config

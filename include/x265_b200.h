@@ -1,4 +1,4 @@
-/* include/x265_b200.h -- C ABI of libx265cu.so, the B200-native (sm_100a) implementation of x265's
+/* include/x265_b200.h -- C ABI of libx265cu.so, the H100-native (sm_90a) implementation of x265's
  * block-primitive hot path.  Plain C: pointers and sizes only, no CUDA/torch types.
  *
  * Two levels, both replacing entries of the reference's EncoderPrimitives table

@@ -22,7 +22,7 @@ W, H = 3840, 2160
 FRAMES = 24          # one launch covers a lookahead-window-sized batch: 24 stacked 2160p frames (~200 MB per plane)
 
 
-SINGLE = False       # --single: every primitive runs exactly once (the ncu dram-bytes pass: profiles/r2_final.sh)
+SINGLE = False       # --single: every primitive runs exactly once (a pass for a profiler)
 
 
 def timed(lib, flush, fn, reps):
@@ -58,7 +58,7 @@ def run(lib, depth=8, reps=7, frames=FRAMES, quiet=False, only=None):
     H = 2160
     es = 1 if depth == 8 else 2
     pdt = np.uint8 if depth == 8 else np.uint16
-    peak = 6567.1
+    peak = 3350.0          # H100 SXM data sheet, HBM3
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:

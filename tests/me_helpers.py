@@ -162,10 +162,11 @@ def run_both_chroma(O, R, depth, rng, w, h, method, subme, smooth, merange, qp=3
     return (cr, int(out_r[0]), int(out_r[1])), (co, int(out_o[0]), int(out_o[1]))
 
 
-def run_both_sea(O, R, depth, rng, w, h, subme, smooth, merange, qp=30):
+def run_both_sea(O, R, depth, rng, w, h, subme, smooth, merange, qp=30, check=None):
     """X265_SEA (motion.cpp:1242-1395) through the real MotionEstimate with the 12 integral planes FrameFilter::computeMEIntegral
     would hand it (x265ref_build_integral: the real integral_init primitives) and through the oracle (orc_build_integral +
-    method 4); also checks the two sets of planes against each other over the region the search can touch."""
+    method 4); also checks the two sets of planes against each other over the region the search can touch (with
+    check(ref_planes, oracle_planes) when given)."""
     mx = (1 << depth) - 1
     W, H, margin = 256, 192, 96
     lam = R.x265ref_lambda(qp)
@@ -184,8 +185,11 @@ def run_both_sea(O, R, depth, rng, w, h, subme, smooth, merange, qp=30):
     R.x265ref_build_integral(ptr(refb, org), stride, H // 64, arr_r)
     O.orc_build_integral(ptr(refb, org), stride, H // 64, arr_o)
     rows = slice(margin - 79, margin + H + 78)
-    for a, b in zip(ipl_r, ipl_o):
-        assert np.array_equal(a[rows], b[rows])
+    if check:
+        check([a[rows] for a in ipl_r], [b[rows] for b in ipl_o])
+    else:
+        for a, b in zip(ipl_r, ipl_o):
+            assert np.array_equal(a[rows], b[rows])
     bx = int(rng.integers(0, (W - w) // 4 + 1)) * 4; by = int(rng.integers(0, (H - h) // 4 + 1)) * 4
     offset = org + by * stride + bx
     qmvp = (int(rng.integers(-40, 41)), int(rng.integers(-40, 41)))

@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: libx265cu.so builds for sm_100a, loads without a GPU and
+"""CPU-side checks of the drop-in boundary: libx265cu.so builds for sm_90a, loads without a GPU and
 exports every symbol include/x265_b200.h declares; compute entry points refuse to run without CUDA
 (no CPU fallback)."""
 import ctypes as C

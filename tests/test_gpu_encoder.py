@@ -31,7 +31,8 @@ def write_cif(path, frames):
 @pytest.mark.timeout(900)
 def test_encoder_bitstream_equals_c_table(tmp_path):
     if not os.path.exists(CLI):
-        pytest.skip("oracle/_ref/x265_ref_cuda not built (make -C oracle -f Makefile.ref encoder_cuda)")
+        pytest.skip("oracle/_ref/x265_ref_cuda not built: the encoder is linked from the reference's sources, so it exists only "
+                    "where build() had them (make -C oracle -f Makefile.ref encoder_cuda)")
     frames = 3
     yuv = str(tmp_path / "cif.yuv")
     write_cif(yuv, frames)

@@ -16,7 +16,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def test_reference_testbench(depth, seed):
     exe = os.path.join(ROOT, "oracle", "_ref", "testbench_cuda%d" % depth)
     if not os.path.exists(exe):
-        pytest.skip("oracle/_ref/testbench_cuda not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/testbench_cuda%d not built: it links the reference's own harness sources, so it exists only "
+                    "where build() had them; test_gpu_table.py compares the same entries with the oracle, and test_oracle_vs_ref.py "
+                    "the oracle with the reference's stored results" % depth)
     r = subprocess.run([exe, str(seed)], capture_output=True, text=True, timeout=900)
     tail = (r.stdout[-1500:] + r.stderr[-1500:])
     assert r.returncode == 0, tail

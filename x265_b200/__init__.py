@@ -1,4 +1,4 @@
-"""x265_b200 -- B200-native (sm_100a) block-primitive engine behind x265's EncoderPrimitives table.
+"""x265_b200 -- H100-native (sm_90a) block-primitive engine behind x265's EncoderPrimitives table.
 
 The product is libx265cu.so (C ABI in include/x265_b200.h).  This package is the thin Python host
 mirror used by tests and bench.py: it loads the library with ctypes and exposes the per-call table

@@ -1,4 +1,4 @@
-"""Builds libx265cu.so (hand-written sm_100a CUDA, single translation unit) in-tree with nvcc."""
+"""Builds libx265cu.so (hand-written sm_90a CUDA, single translation unit) in-tree with nvcc."""
 import os
 import subprocess
 import sys
@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libx265cu.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -142,7 +142,7 @@ __device__ __forceinline__ void blk_store8(void* __restrict__ p, int bytes, cons
 
 // one block per job (grid-stride over jobs), threads stride over the w*h elements.  OPT >= 0: the operation as a compile-time
 // constant (the hot element-wise ops get their own instantiation: with a run-time `op` the per-element switch of
-// blockop_value survives in the unrolled loop -- sub_ps ran at 38 % of the HBM roofline); OPT = -1: any op.
+// blockop_value survives in the unrolled loop); OPT = -1: any op.
 template <typename P, int OPT>
 __global__ void __launch_bounds__(256) k_blockop(int op_rt, void* __restrict__ D, const void* __restrict__ A, const void* __restrict__ B,
                                                  const x265cu_blk_job* __restrict__ jobs, int n)

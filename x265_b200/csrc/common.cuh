@@ -1,4 +1,4 @@
-// x265_b200/csrc/common.cuh -- shared declarations for the sm_100a kernels and the C ABI.
+// x265_b200/csrc/common.cuh -- shared declarations for the sm_90a kernels and the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -63,6 +63,6 @@ __constant__ int16_t c_chromaFilter[8][4] = {
 // transform matrices, generated on the host at context creation (transform.cuh: build_dct_tables)
 __constant__ int8_t c_dct[4][32 * 32];   // [log2N-2][k*N + j]
 // the same matrices in GLOBAL memory for lane-indexed reads (a constant-bank access with 32 different addresses is
-// replayed 32 times: the tensor-core transform's fragment set-up spent ~100 us per launch in such reads)
+// replayed 32 times, which the tensor-core transform's fragment set-up would pay on every TU)
 __device__ int8_t d_dct[4][32 * 32];
 __constant__ int8_t c_dst4[16];

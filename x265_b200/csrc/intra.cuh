@@ -130,8 +130,8 @@ __global__ void __launch_bounds__(256) k_intra_pred(int N, const P* __restrict__
     }
 }
 
-// one WARP per neighbour array (4N+1 <= 129 elements): no shared staging, no CTA barriers; a CTA per job with two
-// __syncthreads for 65 elements ran at 3-5 % of the HBM roofline on frame-sized lists
+// one WARP per neighbour array (4N+1 <= 129 elements): no shared staging, no CTA barriers (a CTA per job would pay two
+// __syncthreads for 65 elements)
 template <typename P>
 __global__ void __launch_bounds__(256) k_intra_filter(int N, const P* __restrict__ nb, P* __restrict__ filt, int64_t pitch, int n)
 {
@@ -231,8 +231,7 @@ __global__ void __launch_bounds__(256) k_intra_allangs_cta(int N, const P* __res
 
 // all-angs on packed pixels: same per-pixel arithmetic as k_intra_allangs_cta, issued 4 (8-bit) / 2 (16-bit) pixels per word.
 // The CTA kernel above spends ~45 instructions per 4 pixels (two shared loads, two IMADs, shift and select per pixel, the
-// packing) and keeps half a warp idle on a 16x16 block (a mode has 16 row units there): 17 % (8-bit) / 33 % (10-bit) of the
-// HBM roofline, issue bound.  Here
+// packing) and keeps half a warp idle on a 16x16 block (a mode has 16 row units there): issue bound.  Here
 //   * neighbours and the projected reference row are kept as PIXELS in shared memory, a work item is a 16-byte piece of an
 //     output row (a whole row up to 16 / 8 pixels): UW + 2 aligned words, funnel shifts to the item's byte phase, then one
 //     DP4A (bytes p[k], p[k+1] against the weights (32 - f, f), + 16 in the accumulator) or DP2A per pixel and one shift;

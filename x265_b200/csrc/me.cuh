@@ -64,7 +64,7 @@ template <typename P> __device__ __forceinline__ int sad_word(uint32_t a, uint32
 {
     return sizeof(P) == 1 ? (int)(__vsadu4(a, b) + (uint32_t)acc) : (int)(__vsadu2(a, b) + (uint32_t)acc);
 }
-// SAD of N (<= 16) words.  8-bit: N VABSDIFF4 with accumulate.  16-bit: sm_100a has no packed absolute-difference-and-add
+// SAD of N (<= 16) words.  8-bit: N VABSDIFF4 with accumulate.  16-bit: sm_90a has no packed absolute-difference-and-add
 // for halves (__vsadu2 is ~8 instructions); max - min per half IS native (VIMNMX.U16x2) and cannot borrow, so the N packed
 // differences are summed in the two 16-bit lanes (<= 16 * 1023 each for 10-bit pixels, <= 16 * 4095 for 12-bit) and folded
 // once: about 3 instructions per word instead of 8.
@@ -215,7 +215,7 @@ __device__ __forceinline__ int me_eval_points(const MeCtx<P>& c, int n, int px, 
 
 
 // tile distortions kept out of line: the job loop is instruction-cache bound, one copy of the unrolled
-// Hadamard instead of six is worth more than the call overhead (measured: profiles/me_r1 notes)
+// Hadamard instead of six is worth more than the call overhead
 template <typename PA, typename PB>
 __device__ __forceinline__ int me_tile8x4(const PA* pf, int sf, const PB* pp, int sp)
 {
@@ -1048,8 +1048,8 @@ __device__ __forceinline__ void me_chroma_hsum4(const P* __restrict__ p, uint32_
 //   yf == 0 is excluded below only for 10-bit horizontal-only phases, where hps drops two bits that hpp keeps;
 //   xf == 0: mid = 64 p - 8192 (8-bit) / 16 p - 8192 (10-bit) is exact, so vsp gives (sum(c p) + 32) >> 6 = filter_vpp;
 //   xf == yf == 0: the pixel itself.
-// Lanes of a pass hold candidates of different phases: a single path means no divergence and a small body (the kernels
-// with this term ran at a 60 % instruction-cache hit rate with the four-way version).
+// Lanes of a pass hold candidates of different phases: a single path means no divergence and a small body (a four-way
+// version of this term made the kernels miss the instruction cache).
 template <typename P>
 __device__ __noinline__ int me_chroma_had4x4(const P* __restrict__ f, const P* __restrict__ r, int stride, int xf, int yf)
 {
@@ -1107,7 +1107,7 @@ __device__ __noinline__ int me_chroma_had4x4(const P* __restrict__ f, const P* _
 }
 
 // position of the (n + 1)-th set bit of `mask` (n < popc(mask)): five halving steps on population counts (__fns is a
-// long software loop: it was 17 % of the instructions of the chroma kernels)
+// long software loop)
 __device__ __forceinline__ int me_nth_set_bit(unsigned mask, int n)
 {
     int pos = 0;
@@ -1658,9 +1658,8 @@ __device__ __forceinline__ void me_make_ctx(MeCtx<P>& c, const x265cu_me_job& j,
 
 // Persistent warps with a dynamic job queue (jobs differ by up to 64x in work).  The search is split into
 // launches -- pre-checks (small PUs, other PUs), integer search, sub-pel refinement (small PUs, other PUs) --
-// because the fused body (12.4 K SASS instructions, ~200 KB) thrashes the instruction cache: ncu
-// showed 80 % of the stall samples in `no_instructions` at a 46 % i-cache hit rate, and the un-split sub-pel
-// kernel (8.8 K instructions, both PU classes resident on every SM) still sat at 64 %.  PHASE 0 = all fused
+// because the fused body (12.4 K SASS instructions, ~200 KB) thrashes the instruction cache, and so does an
+// un-split sub-pel kernel (8.8 K instructions, both PU classes resident on every SM).  PHASE 0 = all fused
 // (the lookahead kernel's per-CU call).
 #ifndef ME_MIN_BLOCKS
 #define ME_MIN_BLOCKS 3
@@ -1792,10 +1791,8 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
                        const MeChromaArgs* ch, const MeWinLaunch* win)
 {
     int rc = 0;
-    // shape-sorted job order (geometry.h `order`), measured on B200 at 2160p (profiles/me_r2_ncu.md section 5): it helps kernels
-    // that miss the instruction cache (the chroma sub-pel launches: 24.2 -> 23.2 ms; 36.7 -> 27.6 ms before the column-split
-    // chroma term made them small) and costs the others ~10 % (they lose the raster order's L1 / L2 locality: luma-only
-    // pre-checks 9.1 -> 10.4 ms, chroma pre-checks 9.7 -> 10.9 ms).  X265CU_ME_ORDER = 0: never, 1: chroma sub-pel launches
+    // shape-sorted job order (geometry.h `order`): it helps kernels that miss the instruction cache (the chroma sub-pel
+    // launches) and slows the others (they lose the raster order's L1 / L2 locality).  X265CU_ME_ORDER = 0: never, 1: chroma sub-pel launches
     // only (default), 2: every pre-check / sub-pel launch.
     static const int ordMode = [] { const char* e = getenv("X265CU_ME_ORDER"); return e ? atoi(e) : 1; }();
     const int32_t* ordAll = (win && !lowres) ? win->order : NULL;

@@ -224,8 +224,8 @@ __device__ __forceinline__ int warp_psy(const P* __restrict__ s, int ss, const P
 }
 
 // ---- batched job-list kernel ---------------------------------------------------------------------------------
-// Round 1 ran one warp per job: an 8x8 SATD kept 2 of 32 lanes busy and an 8x8 SAD paid a 5-step reduction for 64 pixels
-// (2-4 % of the HBM roofline on frame-sized lists of small blocks).  Now a warp takes 32 consecutive jobs (one coalesced
+// One warp per job would keep 2 of 32 lanes busy on an 8x8 SATD and pay a 5-step reduction for 64 pixels of an 8x8 SAD.
+// Instead a warp takes 32 consecutive jobs (one coalesced
 // 1 KB read of the records), picks the SUB-GROUP width the largest of them needs -- lanes per job = pow2ceil(work units),
 // units = 8x4 tiles for SATD, 8x8 tiles for SA8D / PSY, 16-pixel groups for the element-wise costs -- and runs
 // 32 / width jobs side by side per pass; results go back to the lane that read the job, so the 32 outputs are one

@@ -196,8 +196,8 @@ __global__ void __launch_bounds__(256) k_transform_mma(const int16_t* __restrict
             }
             __syncwarp();
             // the NEXT TU's coefficients are requested now and land while this TU is transformed (one warp per TU is a long
-            // dependent chain: load -> tile -> fragments -> 2 x MMA passes -> stores; without the prefetch the inverse sat at
-            // ~57 % of the HBM roofline whatever its access patterns were)
+            // dependent chain: load -> tile -> fragments -> 2 x MMA passes -> stores, which the prefetch overlaps with the
+            // loads)
             if (PRE && in16 && tu + nwarps < n)
             {
                 const int16_t* sn = src + (int64_t)(tu + nwarps) * N * N;
