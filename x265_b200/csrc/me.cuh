@@ -1715,17 +1715,20 @@ template <typename P, int PHASE, int CLS>
 __global__ void __launch_bounds__(256, CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS) k_me_chroma(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride,
                                                            MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs, int n,
                                                            int32_t* __restrict__ out, MeState* __restrict__ state, int* __restrict__ counter,
+                                                           const int32_t* __restrict__ list = nullptr, const int* __restrict__ list_n = nullptr,
                                                            const int32_t* __restrict__ order = nullptr, int order0 = 0)
 {
     extern __shared__ unsigned char me_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     MeShared* sm = (MeShared*)me_smem + warp;
+    if (list) n = *list_n;                             // the jobs list[0 .. *list_n) (see k_me)
     for (;;)
     {
         int jid = 0;
         if (lane == 0) jid = atomicAdd(counter, 1);
         jid = __shfl_sync(0xffffffffu, jid, 0);
         if (jid >= n) break;
+        if (list) jid = list[jid];
         if (order) jid = order[jid] - order0;          // shape-sorted job order (see k_me)
         const x265cu_me_job j = jobs[jid];
         MeCtx<P> c;
@@ -1743,14 +1746,15 @@ __global__ void __launch_bounds__(256, CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS)
 template <typename P, int PHASE, int CLS>
 static int launch_me_chroma_phase(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs& ch,
                                   const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, MeState* state, int* counter,
-                                  const int32_t* order = NULL, int order0 = 0)
+                                  const int32_t* list = NULL, const int* list_n = NULL, const int32_t* order = NULL, int order0 = 0)
 {
     const int threads = 256, warps = threads / 32;
     const size_t smem = sizeof(MeShared) * warps;
     int blocks = ctx->sm_count * (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS);
     int need = (n + warps - 1) / warps;
     if (blocks > need) blocks = need;
-    k_me_chroma<P, PHASE, CLS><<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ch, mvcost, jobs, n, out, state, counter, order, order0);
+    k_me_chroma<P, PHASE, CLS><<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ch, mvcost, jobs, n, out, state, counter,
+                                                                       list, list_n, order, order0);
     CU_LAUNCH_CHECK(ctx);
     return 0;
 }
@@ -1784,6 +1788,9 @@ struct MeWinLaunch
 template <typename P>
 static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, const uint16_t* mvcost, const x265cu_me_job* jobs,
                             MeState* st, const MeWinLaunch& w);
+template <typename P>
+static int launch_me_precheck_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs* ch,
+                                     const uint16_t* mvcost, const x265cu_me_job* jobs, MeState* st, const MeWinLaunch& w, int* left_count, int32_t* left_list);
 
 template <typename P>
 static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres,
@@ -1799,15 +1806,23 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
     const int32_t* ord = ordMode >= 2 ? ordAll : NULL;                       // pre-checks, luma-only sub-pel
     const int32_t* ord3 = (ordMode >= 2 || (ordMode == 1 && ch)) ? ordAll : NULL;   // chroma sub-pel
     const int ord0 = win ? win->job0 : 0;
+    // pre-checks: with job groups, the 16x16 cells out of shared per-cell tables (me_window.cuh) and only the other jobs
+    // through the per-PU kernels; the window search's leftover list is free until the integer search and carries them
+    const int32_t* pre = NULL; const int* pre_n = NULL; const int32_t* ord1 = ord;
+    if (win && !lowres)
+    {
+        rc |= launch_me_precheck_groups<P>(ctx, fenc, fstride, refs, rstride, ch, mvcost, jobs, st, *win, win->left_count, win->left_list);
+        pre = win->left_list; pre_n = win->left_count; ord1 = NULL;
+    }
     if (ch)
     {
-        rc |= launch_me_chroma_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 0, ord, ord0);
-        rc |= launch_me_chroma_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 1, ord, ord0);
+        rc |= launch_me_chroma_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 0, pre, pre_n, ord1, ord0);
+        rc |= launch_me_chroma_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 1, pre, pre_n, ord1, ord0);
     }
     else
     {
-        rc |= launch_me_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 0, NULL, NULL, ord, ord0);
-        rc |= launch_me_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 1, NULL, NULL, ord, ord0);
+        rc |= launch_me_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 0, pre, pre_n, ord1, ord0);
+        rc |= launch_me_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 1, pre, pre_n, ord1, ord0);
     }
     CU_CHECK(cudaEventRecord(ctx->me_ev[1], ctx->stream));
     if (win && !lowres)
@@ -1821,8 +1836,8 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
     CU_CHECK(cudaEventRecord(ctx->me_ev[2], ctx->stream));
     if (ch)
     {
-        rc |= launch_me_chroma_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 3, ord3, ord0);
-        rc |= launch_me_chroma_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 4, ord3, ord0);
+        rc |= launch_me_chroma_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord3, ord0);
+        rc |= launch_me_chroma_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord3, ord0);
     }
     else
     {

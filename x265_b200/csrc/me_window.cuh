@@ -852,3 +852,223 @@ static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, cons
     }
     return 0;
 }
+
+// ---- pre-checks of the 16x16 cell groups (phase 1, motion.cpp:771-814) -------------------------------------------------
+// Every job of a cell takes its MVP and both candidates from the field block of the cell (k_build_me_jobs), so -- unless a
+// picture-edge clamp of mvmin / mvmax moves a clip -- all of them evaluate the same positions: the clipped MVP, its full-pel
+// rounding, MV 0 and the candidates.  A PU's SAD is the sum of its 4x4 blocks' SADs, and its chroma SATD is the sum of 4x4
+// (chroma width 4) or 8x4 (width 8) tiles, an 8x4 tile being the two un-halved 4x4 Hadamard sums added and halved
+// (pixel.cpp:239-297).  The interpolated prediction at a position does not depend on the block.  So one warp per cell
+// evaluates each position ONCE over the whole 16x16 cell into a table of 4x4 quantities and folds every job from it, one
+// lane per job, exactly as me_phase1 does.  A job whose clipped positions differ from the cell's first job goes to
+// `left_list` for the per-PU kernels, and so do all jobs of the CU 64 / CU 32 groups (CELL == false launches).
+struct MePreTab
+{
+    int16_t mid[(16 + 7) * 16];            // hps(rowExt) rows of an hv position (me_subpel_small_t's layout for a 16x16 PU)
+    int lum[5][16];                        // luma 4x4 SADs: MVP, its full-pel rounding, MV 0, candidate 0, candidate 1
+    int chr[3][8];                         // un-halved chroma 4x4 Hadamard sums [MVP, cand 0, cand 1][Cb tiles 0-3, Cr tiles 0-3]
+};
+
+template <typename P, bool CHROMA>
+__global__ void __launch_bounds__(256) k_me_precheck_cell(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride,
+                                                          MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs,
+                                                          const MeGroup* __restrict__ groups, int ngroups, const int32_t* __restrict__ grp_jobs, int job0,
+                                                          int cell, MeState* __restrict__ state, int* __restrict__ left_count, int32_t* __restrict__ left_list)
+{
+    constexpr int DEPTH = PixTraits<P>::depth;
+    __shared__ __align__(16) MePreTab tabs[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gi = blockIdx.x * 8 + warp;
+    if (gi >= ngroups) return;
+    const MeGroup g = groups[gi];
+    if (!cell)
+    {
+        int base = 0;
+        if (lane == 0) base = atomicAdd(left_count, g.count);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        for (int i = lane; i < g.count; i += 32) left_list[base + i] = grp_jobs[g.first + i] - job0;
+        return;
+    }
+    MePreTab& t = tabs[warp];
+
+    // the cell's positions: those of its first job
+    const x265cu_me_job j0 = jobs[grp_jobs[g.first] - job0];
+    const int qminx = j0.mvmin[0] * 4, qminy = j0.mvmin[1] * 4, qmaxx = j0.mvmax[0] * 4, qmaxy = j0.mvmax[1] * 4;
+    const int pmvx = max(min((int)j0.qmvp[0], qmaxx), qminx), pmvy = max(min((int)j0.qmvp[1], qmaxy), qminy);
+    const int bmx = (pmvx + 2) >> 2, bmy = (pmvy + 2) >> 2;
+    const int c0x = max(min((int)j0.mvc[0], qmaxx), qminx), c0y = max(min((int)j0.mvc[1], qmaxy), qminy);
+    const int c1x = max(min((int)j0.mvc[2], qmaxx), qminx), c1y = max(min((int)j0.mvc[3], qmaxy), qminy);
+    const int ncand = j0.numCand;
+    const bool frac = ((pmvx & 3) | (pmvy & 3)) != 0, nonzero = (pmvx | pmvy) != 0;
+    const bool v0 = ncand > 0 && (c0x | c0y) && !(c0x == pmvx && c0y == pmvy);
+    const bool v1 = ncand > 1 && (c1x | c1y) && !(c1x == pmvx && c1y == pmvy);
+    const int oy0 = j0.offset / fstride, ox0 = j0.offset - oy0 * fstride;
+    const int cx = ox0 & ~15, cy = oy0 & ~15;
+    const ptrdiff_t coff = (ptrdiff_t)cy * fstride + cx;
+    const P* rb = refs[j0.ref] + coff;
+    const P* fb = fenc + coff;
+
+    // ---- luma: lane = (8-pixel segment, row) of the cell, as me_subpel_small_t maps a 16x16 PU ----
+    const int row = lane & 15, seg = lane >> 4;
+#pragma unroll 1
+    for (int k = 0; k < 5; k++)
+    {
+        if ((k == 1 && !frac) || (k == 2 && !nonzero) || (k == 3 && !v0) || (k == 4 && !v1)) continue;
+        const int qx = k == 0 ? pmvx : k == 1 ? bmx * 4 : k == 2 ? 0 : k == 3 ? c0x : c1x;
+        const int qy = k == 0 ? pmvy : k == 1 ? bmy * 4 : k == 2 ? 0 : k == 3 ? c0y : c1y;
+        const int xf = qx & 3, yf = qy & 3;
+        const P* r = rb + (qx >> 2) + (ptrdiff_t)(qy >> 2) * rstride;
+        int pr[8];
+        if (xf && yf)
+        {
+            __syncwarp();
+            for (int tk = lane; tk < (16 + 7) * 2; tk += 32)
+            {
+                const int mrow = tk >> 1, sg = tk & 1;
+                int sum[8];
+                me_hrow<P, 8>(r + (ptrdiff_t)(mrow - 3) * rstride + sg * 8, xf, sum);
+                uint32_t pk[4];
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+                    pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
+                *(uint4*)(t.mid + mrow * 16 + sg * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+            }
+            __syncwarp();
+            me_vmid<8>(t.mid + row * 16 + seg * 8, 16, yf, pr);
+#pragma unroll
+            for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 2);
+        }
+        else
+        {
+            const P* rr = r + (ptrdiff_t)row * rstride + seg * 8;
+            if (!(xf | yf)) me_ld_px<P, 8>(rr, pr);
+            else if (!yf)
+            {
+                me_hrow<P, 8>(rr, xf, pr);
+#pragma unroll
+                for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 0);
+            }
+            else
+            {
+                me_vcol<P, 8>(rr - 3 * (ptrdiff_t)rstride, rstride, yf, pr);
+#pragma unroll
+                for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 0);
+            }
+        }
+        int fv[8];
+        me_ld_px<P, 8>(fb + (ptrdiff_t)row * fstride + seg * 8, fv);
+        int sl = 0, sr = 0;
+#pragma unroll
+        for (int x = 0; x < 4; x++) { sl += abs(fv[x] - pr[x]); sr += abs(fv[x + 4] - pr[x + 4]); }
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) { sl += __shfl_xor_sync(0xffffffffu, sl, o); sr += __shfl_xor_sync(0xffffffffu, sr, o); }
+        if ((row & 3) == 0) { t.lum[k][(row >> 2) * 4 + seg * 2] = sl; t.lum[k][(row >> 2) * 4 + seg * 2 + 1] = sr; }
+    }
+    // ---- chroma: lane = (position, plane, 4x4 tile) of the cell's 8x8 chroma block ----
+    if (CHROMA && lane < 24)
+    {
+        const int k = lane >> 3, cr = (lane >> 2) & 1, tt = lane & 3;
+        const int qx = k == 0 ? pmvx : k == 1 ? c0x : c1x, qy = k == 0 ? pmvy : k == 1 ? c0y : c1y;
+        if (k == 0 || (k == 1 && v0) || (k == 2 && v1))
+        {
+            const ptrdiff_t o = (ptrdiff_t)(cy >> 1) * ch.cstride + (cx >> 1) + (ptrdiff_t)((tt >> 1) * 4) * ch.cstride + (tt & 1) * 4;
+            const P* f = (const P*)(cr ? ch.fencCr : ch.fencCb) + o;
+            const P* r = ((const P* const*)(cr ? ch.refCr : ch.refCb))[j0.ref] + o + (qx >> 3) + (ptrdiff_t)(qy >> 3) * ch.cstride;
+            t.chr[k][cr * 4 + tt] = me_chroma_had4x4<P>(f, r, ch.cstride, qx & 7, qy & 7);
+        }
+    }
+    __syncwarp();
+
+    // ---- fold: one lane per job (a cell holds up to 33 jobs with AMP) ----
+    for (int base = 0; base < g.count; base += 32)
+    {
+        const int slot = base + lane;
+        const bool live = slot < g.count;
+        const int jid = live ? grp_jobs[g.first + slot] - job0 : 0;
+        const x265cu_me_job j = jobs[jid];
+        const int jqminx = j.mvmin[0] * 4, jqminy = j.mvmin[1] * 4, jqmaxx = j.mvmax[0] * 4, jqmaxy = j.mvmax[1] * 4;
+        const bool same = j.numCand == ncand && ncand <= 2 &&
+                          max(min((int)j.qmvp[0], jqmaxx), jqminx) == pmvx && max(min((int)j.qmvp[1], jqmaxy), jqminy) == pmvy &&
+                          (ncand < 1 || (max(min((int)j.mvc[0], jqmaxx), jqminx) == c0x && max(min((int)j.mvc[1], jqmaxy), jqminy) == c0y)) &&
+                          (ncand < 2 || (max(min((int)j.mvc[2], jqmaxx), jqminx) == c1x && max(min((int)j.mvc[3], jqmaxy), jqminy) == c1y));
+        const unsigned lost = __ballot_sync(0xffffffffu, live && !same);
+        if (lost)
+        {
+            int lb = 0;
+            if (lane == 0) lb = atomicAdd(left_count, __popc(lost));
+            lb = __shfl_sync(0xffffffffu, lb, 0);
+            if ((lost >> lane) & 1u) left_list[lb + __popc(lost & ((1u << lane) - 1u))] = jid;
+        }
+        if (!live || !same) continue;
+        const int py = j.offset / fstride, px = j.offset - py * fstride;
+        const int bx0 = (px - cx) >> 2, by0 = (py - cy) >> 2, bw = j.pw >> 2, bh = j.ph >> 2;
+        int L[5];
+#pragma unroll
+        for (int k = 0; k < 5; k++)
+        {
+            int s = 0;
+            for (int by = by0; by < by0 + bh; by++)
+                for (int bx = bx0; bx < bx0 + bw; bx++) s += t.lum[k][by * 4 + bx];
+            L[k] = s;
+        }
+        int C[3] = { 0, 0, 0 };
+        if (CHROMA && j.subme > 2 && !(j.pw & 7) && !(j.ph & 7))
+        {   // chroma block (w/2) x (h/2): 8x4 tiles when its width is 8, else 4x4 tiles; each tile halved on its own
+            const int tx0 = (px - cx) >> 3, ty0 = (py - cy) >> 3, th = j.ph >> 3;
+#pragma unroll
+            for (int k = 0; k < 3; k++)
+#pragma unroll
+                for (int cr = 0; cr < 2; cr++)
+                    for (int ty = ty0; ty < ty0 + th; ty++)
+                    {
+                        const int* s = &t.chr[k][cr * 4 + ty * 2];
+                        C[k] += j.pw == 16 ? (s[0] + s[1]) >> 1 : s[tx0] >> 1;
+                    }
+        }
+        // me_phase1's fold
+        const int mvpx = j.qmvp[0], mvpy = j.qmvp[1];
+        int bprecost = L[0] + C[0], bcost = bprecost, bestprex = pmvx, bestprey = pmvy, jbmx = bmx, jbmy = bmy;
+        if (frac) bcost = L[1] + (uint16_t)(__ldg(mvcost + (bmx * 4 - mvpx)) + __ldg(mvcost + (bmy * 4 - mvpy)));
+        if (nonzero)
+        {
+            const int cz = L[2] + (uint16_t)(__ldg(mvcost - mvpx) + __ldg(mvcost - mvpy));
+            if (cz < bcost) { bcost = cz; jbmx = 0; jbmy = max(min(0, (int)j.mvmax[1]), (int)j.mvmin[1]); }
+        }
+        int cbest = 0x7fffffff, cbx = 0, cby = 0;
+        if (v0)
+        {
+            const int cost = L[3] + C[1] + (uint16_t)(__ldg(mvcost + (c0x - mvpx)) + __ldg(mvcost + (c0y - mvpy)));
+            cbest = cost; cbx = c0x; cby = c0y;
+        }
+        if (v1)
+        {
+            const int cost = L[4] + C[2] + (uint16_t)(__ldg(mvcost + (c1x - mvpx)) + __ldg(mvcost + (c1y - mvpy)));
+            if (cost < cbest) { cbest = cost; cbx = c1x; cby = c1y; }
+        }
+        if (cbest < bprecost) { bprecost = cbest; bestprex = cbx; bestprey = cby; }
+        MeState st;
+        st.bmx = jbmx; st.bmy = jbmy; st.bcost = bcost; st.bprecost = bprecost; st.bestprex = bestprex; st.bestprey = bestprey;
+        state[jid] = st;
+    }
+}
+
+// Pre-checks of a frame slice's groups: cells out of shared tables, every other job (CU 64 / CU 32 groups, cells' jobs with
+// other clips) appended to `left_list` (count in *left_count, zeroed here) for the per-PU kernels.
+template <typename P>
+static int launch_me_precheck_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs* ch,
+                                     const uint16_t* mvcost, const x265cu_me_job* jobs, MeState* st, const MeWinLaunch& w, int* left_count, int32_t* left_list)
+{
+    CU_CHECK(cudaMemsetAsync(left_count, 0, sizeof(int), ctx->stream));
+    const MeChromaArgs none = {};
+    for (int cls = 0; cls < 3; cls++)
+    {
+        if (w.ngroups[cls] <= 0) continue;
+        const int blocks = (w.ngroups[cls] + 7) / 8;
+        if (ch) k_me_precheck_cell<P, true><<<blocks, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, *ch, mvcost, jobs,
+                                                                            (const MeGroup*)w.groups[cls], w.ngroups[cls], w.grp_jobs[cls], w.job0, cls == 2, st, left_count, left_list);
+        else    k_me_precheck_cell<P, false><<<blocks, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, none, mvcost, jobs,
+                                                                             (const MeGroup*)w.groups[cls], w.ngroups[cls], w.grp_jobs[cls], w.job0, cls == 2, st, left_count, left_list);
+        CU_LAUNCH_CHECK(ctx);
+    }
+    return 0;
+}
