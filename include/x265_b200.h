@@ -223,7 +223,8 @@ typedef struct x265cu_analyser x265cu_analyser;
 typedef struct {
     int width, height, depth, numRefs;
     int method, subme, merange, rect;     /* X265_*_SEARCH, subpel refine level, range, rect PUs */
-    int qp; double lambda;                /* quant QP; mvcost lambda (x265_lambda_tab[qp]) */
+    int qp; double lambda;                /* quant QP, 0..51 + 6 * (depth - 8) (the slice QP plus QP_BD_OFFSET);
+                                             mvcost lambda (x265_lambda_tab[qp]), finite and >= 0 */
     int amp;                              /* AMP PUs (2NxnU/nD, nLx2N/nRx2N at CU >= 16; presets slower+, param.cpp:494-520) */
 } x265cu_analysis_params;
 typedef struct {                          /* host destinations (any may be NULL) */
@@ -233,8 +234,8 @@ typedef struct {                          /* host destinations (any may be NULL)
 } x265cu_analysis_out;
 /* Returns NULL, with the reason in x265cu_last_error(), for parameters the device cannot run as the reference does:
  * method not 0 (DIA), 1 (HEX), 3 (STAR) or 5 (FULL); merange outside 0..127 (x265cu_me_job holds it in 8 bits); subme
- * outside 0..7; width or height not a positive multiple of 8.  Also NULL without a message when numRefs is not 1..16 or
- * depth not 8 or 10. */
+ * outside 0..7; width or height not a positive multiple of 8; qp outside 0..51 + 6 * (depth - 8), the QPs the quantiser
+ * has; lambda negative, infinite or NaN.  Also NULL without a message when numRefs is not 1..16 or depth not 8 or 10. */
 x265cu_analyser* x265cu_analyser_create(x265cu_ctx*, const x265cu_analysis_params*);
 void x265cu_analyser_destroy(x265cu_analyser*);
 int x265cu_analyser_counts(x265cu_analyser*, int* njobs, int* ncu, int* ntu, int64_t* ncoef, int* stride);

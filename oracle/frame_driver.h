@@ -15,6 +15,7 @@
 #ifndef X265_FRAME_DRIVER_H
 #define X265_FRAME_DRIVER_H
 #include "frame_spec.h"
+#include <assert.h>
 #include <pthread.h>
 #include <stdlib.h>
 #include <string.h>
@@ -150,6 +151,8 @@ static void drv_resid_one(drv_frame* f, int c)
     /* TUs */
     const int T = S > 32 ? 32 : S;
     const int lg = T == 32 ? 5 : (T == 16 ? 4 : (T == 8 ? 3 : 2));
+    /* the quantiser's QPs are 0..51 + QP_BD_OFFSET (quant.cpp:224); a negative QP would index the tables at rem < 0 */
+    assert(p->qp >= 0 && p->qp <= 51 + 6 * (DRV_DEPTH - 8));
     const int per = p->qp / 6, rem = p->qp % 6;
     static const int quantScales[6] = { 26214, 23302, 20560, 18396, 16384, 14564 };   /* scalinglist.cpp:129 */
     static const int invQuantScales[6] = { 40, 45, 51, 57, 64, 72 };                  /* scalinglist.cpp:130 */

@@ -54,3 +54,21 @@ def test_mvcost_table_matches_oracle():
         b = np.zeros(2 * 4096 + 1, np.uint16)
         O.orc_mvcost_table(C.c_double(lam), 4096, ptr(b))
         assert np.array_equal(a, b)
+
+
+def test_mvcost_table_every_qp():
+    """The host builder at the analyser's range (+-65536) for the lambda of every QP up to QP_MAX_MAX, at 8 and 10 bit:
+    from 0.25 to the 10-bit lambdas whose tables reach the cap of 32767."""
+    import numpy as np
+    import x265_b200
+    from common import load_oracle, ptr
+    from frame_helpers import lambda_for, MVRANGE
+    lib = x265_b200.load(need_gpu=False)
+    O = load_oracle(8)
+    for depth in (8, 10):
+        for qp in range(70):
+            lam = lambda_for(qp, depth)
+            a = lib.mvcost_table(lam, MVRANGE)
+            b = np.zeros(2 * MVRANGE + 1, np.uint16)
+            O.orc_mvcost_table(C.c_double(lam), MVRANGE, ptr(b))
+            assert np.array_equal(a, b), (depth, qp, lam)

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from common import load_oracle
-from frame_helpers import Workload, cpu_analyse, lambda_for, MVRANGE
+from frame_helpers import Workload, cpu_analyse, lambda_for, assert_qp_case_reaches, MVRANGE, QP_CASES
 from me_helpers import mvcost_table
 from ref_results import RefResults
 
@@ -90,6 +90,22 @@ def test_frame_driver_search_space(name, depth, opts, request):
         assert outside_x(a["jobs"]) > 0.9 * a["njobs"]
     if opts.get("content") == "full10":
         assert wl.fenc.min() == 0 and wl.fenc.max() == 1023 and (wl.fenc & 3).any()
+    compare(G, a, wl, tab)
+
+
+@pytest.mark.parametrize("content,depth,qp,chroma", QP_CASES, ids=["%s-%d-qp%d" % c[:3] for c in QP_CASES])
+def test_frame_driver_qp(content, depth, qp, chroma, request):
+    """The frame driver across the quantiser's QP range (frame_helpers.QPS: every qp % 6 and every qp / 6 from 0 to the
+    top), with the mv cost of each QP.  A cut from black ("cut") at every QP: constant white TUs take the DC-only
+    shortcut, 10-bit levels reach the int16 clip at QP 0 and 3, ringing reaches the reconstruction clip, and every SAD
+    ties, so that the mv cost alone decides the searches.  Noise and flat areas with chroma at the lowest and highest QP:
+    full TUs, all-zero TUs and TUs with one nonzero AC level."""
+    G = RefResults(request, depth)
+    O = load_oracle(depth)
+    wl = Workload(200, 136, depth=depth, numRefs=2, method=3, subme=3, merange=57, rect=1, qp=qp, content=content, chroma=chroma)
+    tab = mvcost_table(O, lambda_for(qp, depth))
+    a = cpu_analyse(O, "orc_analyse_frame", wl, tab, threads=4)
+    assert_qp_case_reaches(O, content, wl, a)
     compare(G, a, wl, tab)
 
 

@@ -72,7 +72,8 @@ def oracle_run(O, depth, fenc, refs, stride, jobs, lowres, tab):
 @pytest.mark.parametrize("method", [0, 1, 3, 5])
 @pytest.mark.parametrize("lowres", [0, 1])
 @pytest.mark.parametrize("smooth", [True, False])
-def test_me_batch(cu, depth, method, lowres, smooth):
+def test_me_batch(cu, depth, method, lowres, smooth, lam=None):
+    """lam: the mv cost lambda, by default that of QP 33."""
     O = load_oracle(depth)
     rng = np.random.default_rng(100 + method * 7 + lowres * 3 + depth + smooth)
     W, H, margin = 256, 192, 96
@@ -97,7 +98,8 @@ def test_me_batch(cu, depth, method, lowres, smooth):
         refs = [refb] * 4
     n = 160 if method != 3 else 96
     jobs = build_jobs(rng, W, H, margin, stride, org, n, method, lowres, merange)
-    lam = 11.3137 if depth == 8 else 45.2548
+    if lam is None:
+        lam = 11.3137 if depth == 8 else 45.2548
     tab = mvcost_table(O, lam)
     want = oracle_run(O, depth, fenc, refs, stride, jobs, lowres, tab)
 
@@ -115,6 +117,18 @@ def test_me_batch(cu, depth, method, lowres, smooth):
     assert len(bad) == 0, (len(bad), [(jobs[b].tolist(), got[b].tolist(), want[b].tolist()) for b in bad[:3]])
     for d in [d_fenc, d_table, d_tab, d_jobs, d_out] + d_refs:
         d.free()
+
+
+@pytest.mark.parametrize("depth", [8, 10])
+@pytest.mark.parametrize("method", [0, 1, 3, 5])
+@pytest.mark.parametrize("lowres", [0, 1])
+@pytest.mark.parametrize("smooth", [True, False])
+@pytest.mark.parametrize("qp", ["0", "top"])
+def test_me_batch_qp_extremes(cu, depth, method, lowres, smooth, qp):
+    """The same jobs with the lambda of QP 0 (mv costs of 0 to 2 near the MVP: SAD ties decide the arg-mins) and of the
+    top QP, 51 or 63 at 10 bit (the MVP dominates, and at 10 bit the cost table reaches its cap of 32767)."""
+    from frame_helpers import lambda_for, qp_max
+    test_me_batch(cu, depth, method, lowres, smooth, lam=lambda_for(0 if qp == "0" else qp_max(depth), depth))
 
 
 FAR_RANGES = {0: 57, 1: 57, 3: 92, 5: 8}

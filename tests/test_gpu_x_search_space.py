@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from common import load_oracle
-from frame_helpers import Workload, cpu_analyse, lambda_for, MARGIN_X, MARGIN_Y
+from frame_helpers import Workload, cpu_analyse, lambda_for, run_analyser, assert_frame_equal, MARGIN_X, MARGIN_Y
 from me_helpers import mvcost_table
 
 pytestmark = pytest.mark.gpu
@@ -121,53 +121,31 @@ def _case(name):
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("name,window", PARAMS, ids=["%s-window%s" % p for p in PARAMS])
 def test_search_space(cu, name, window, monkeypatch):
-    import x265_b200
     wl, want = _case(name)
     assert CASES[name][2](wl, want["jobs"]), "the inputs do not reach: " + CASES[name][0]
     monkeypatch.setenv("X265CU_ME_WINDOW", window)
-    p, H, W, qp = wl.params, wl.H, wl.W, 30
-    an = x265_b200.Analyser(cu, W, H, depth=wl.depth, numRefs=p["numRefs"], method=p["method"], subme=p["subme"],
-                            merange=p["merange"], rect=p["rect"], qp=qp, lam=lambda_for(qp, wl.depth), amp=p["amp"])
-    for r, ref in enumerate(wl.refs):
-        an.set_ref(r, ref[MARGIN_Y:MARGIN_Y + H, MARGIN_X:MARGIN_X + W])
-    if wl.chroma:
-        an.enable_chroma()
-        mx, my = MARGIN_X // 2, MARGIN_Y // 2
-
-        def inner(c):
-            return np.ascontiguousarray(c[my:my + H // 2, mx:mx + W // 2])
-        for r in range(len(wl.refs)):
-            an.set_ref_chroma(r, inner(wl.refC[r][0]), inner(wl.refC[r][1]))
-        an.load_chroma(inner(wl.fencC[0]), inner(wl.fencC[1]))
-    an.analyse(np.ascontiguousarray(wl.fenc[MARGIN_Y:MARGIN_Y + H, MARGIN_X:MARGIN_X + W]), wl.field)
-    assert an.njobs == want["njobs"] and an.ncu == want["ncu"]
-    jobs = an.fetch("jobs")
-    assert np.array_equal(jobs, want["jobs"]), "job lists differ"
-    me = an.fetch("me_out").reshape(-1, 4)
-    bad = np.nonzero((me[:, :3] != want["me_out"][:, :3]).any(axis=1))[0]
-    assert len(bad) == 0, (len(bad), len(me), jobs[bad[:4]].tolist(), me[bad[:4]].tolist(), want["me_out"][bad[:4]].tolist())
-    assert np.array_equal(an.cu_ref, want["cu_ref"])
-    assert np.array_equal(an.fetch("coef"), want["coef"])
-    assert np.array_equal(an.cu_numsig, want["cu_numsig"]) and np.array_equal(an.cu_sse, want["cu_sse"])
-    for d in range(4):
-        got = an.fetch("recon%d" % d).reshape(wl.fenc.shape)[MARGIN_Y:MARGIN_Y + H, MARGIN_X:MARGIN_X + W]
-        assert np.array_equal(got, want["recon"][d][MARGIN_Y:MARGIN_Y + H, MARGIN_X:MARGIN_X + W]), "recon depth %d" % d
-    assert np.array_equal(an.intra_cost, want["intra_cost"])
+    an = run_analyser(cu, wl)
+    assert_frame_equal(an, want, wl)
     an.close()
 
 
-# parameters the device cannot run as the reference does: the analyser refuses them
+# parameters the device cannot run as the reference does, or that the quantiser does not have: the analyser refuses them
 REFUSED = [dict(method=2), dict(method=4), dict(method=6), dict(method=-1), dict(merange=128), dict(merange=-1),
-           dict(subme=8), dict(subme=-1), dict(W=0), dict(W=204), dict(H=132), dict(H=-8)]
+           dict(subme=8), dict(subme=-1), dict(W=0), dict(W=204), dict(H=132), dict(H=-8),
+           dict(qp=-1), dict(qp=52), dict(depth=10, qp=-1), dict(depth=10, qp=64), dict(qp=-6),
+           dict(lam=-0.5), dict(lam=float("inf")), dict(lam=float("nan"))]
 
 
 @pytest.mark.parametrize("bad", REFUSED, ids=[",".join("%s=%s" % kv for kv in b.items()) for b in REFUSED])
 def test_analyser_refuses(cu, bad):
     import x265_b200
-    kw = dict(W=64, H=64, method=3, subme=3, merange=57)
+    kw = dict(W=64, H=64, method=3, subme=3, merange=57, depth=8, qp=30, lam=None)
     kw.update(bad)
-    with pytest.raises(RuntimeError, match="x265cu_analyser_create: (search method|merange|subme|width and height)"):
-        x265_b200.Analyser(cu, kw.pop("W"), kw.pop("H"), depth=8, numRefs=1, rect=1, qp=30, **kw)
+    with pytest.raises(RuntimeError, match="x265cu_analyser_create: (search method|merange|subme|width and height|qp|lambda)"):
+        x265_b200.Analyser(cu, kw.pop("W"), kw.pop("H"), numRefs=1, rect=1, **kw)
     # the limits themselves are accepted
-    for ok in (dict(method=5, merange=0, subme=0), dict(method=0, merange=127, subme=7)):
-        x265_b200.Analyser(cu, 64, 64, depth=8, numRefs=1, rect=1, qp=30, **ok).close()
+    for ok in (dict(method=5, merange=0, subme=0), dict(method=0, merange=127, subme=7), dict(qp=0, lam=0.0), dict(qp=51),
+               dict(depth=10, qp=0), dict(depth=10, qp=63, lam=1e6)):
+        kw = dict(depth=8, qp=30)
+        kw.update(ok)
+        x265_b200.Analyser(cu, 64, 64, numRefs=1, rect=1, **kw).close()

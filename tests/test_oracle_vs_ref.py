@@ -24,11 +24,11 @@ class _NoRef:
     oracle's results with the reference's stored ones instead."""
 
     def __init__(self, depth):
-        self._lam = lambda_for(30, depth)
+        self._depth = depth
 
     def x265ref_lambda(self, qp):
-        assert qp == 30
-        return self._lam
+        # equal to the reference's table at every QP (test_mvcost_table)
+        return lambda_for(qp, self._depth)
 
     def __getattr__(self, name):
         class _Call:
@@ -62,15 +62,20 @@ def test_constants(depth, request):
 @pytest.mark.parametrize("depth", DEPTHS)
 def test_mvcost_table(depth, request):
     """The oracle's mv cost table against BitCost's (bitcost.cpp:33-110) over the whole +-2 * BC_MAX_MV range, where far
-    predictors and long searches put their differences; a few QPs."""
+    predictors and long searches put their differences, and lambda_for against x265_lambda_tab: every QP up to QP_MAX_MAX.
+    The 10-bit tables reach BitCost's cap of 32767 from QP 60 on; the 8-bit ones never do."""
     from me_helpers import MVRANGE
     G = RefResults(request, depth)
     O = load_oracle(depth)
-    for qp in (22, 30, 37, 45):
+    capped = []
+    for qp in range(70):
         lam = lambda_for(qp, depth)
         G.same("lambda %d" % qp, lambda: G.R.x265ref_lambda(qp), lam)
         ours = np.zeros(2 * MVRANGE + 1, np.uint16)
         O.orc_mvcost_table(C.c_double(lam), MVRANGE, ours.ctypes.data)
+        assert ours.max() <= 32767
+        if ours.max() == 32767:
+            capped.append(qp)
 
         def ref():
             t = np.zeros(2 * MVRANGE + 1, np.uint16)
@@ -79,6 +84,7 @@ def test_mvcost_table(depth, request):
             G.R.x265ref_mvcost_table(qp, MVRANGE, t.ctypes.data)
             return t
         G.same("table %d" % qp, ref, ours)
+    assert capped == (list(range(60, 70)) if depth == 10 else []), capped
 
 
 @pytest.mark.parametrize("depth", DEPTHS)
@@ -167,6 +173,30 @@ def test_motion_estimate_full_search(depth, request):
                 got.append(o); want.append(r)
                 n += 1
     assert n == 72
+    G.same("results", lambda: want, got)
+
+
+@pytest.mark.parametrize("depth", DEPTHS)
+@pytest.mark.parametrize("method", [0, 1, 3, 5])
+@pytest.mark.parametrize("qp", ["0", "top"])
+def test_motion_estimate_qp(depth, method, qp, request):
+    """The QP extremes of the mv cost: at QP 0 the lambda is 0.25 (8 bit) or 1 (10 bit), so the mv cost near the MVP is
+    0 to 2 and SAD ties decide; at the top QP (51, or 63 at 10 bit) the MVP dominates and the searches stop early.  Every
+    PU size, smooth content."""
+    from frame_helpers import qp_max
+    G, R, O = ref_or_stand_in(request, depth)
+    q = 0 if qp == "0" else qp_max(depth)
+    got, want = [], []
+    rng = np.random.default_rng(900 + 10 * method + q)
+    sizes = [(8, 8), (16, 16), (32, 32), (64, 64), (16, 8), (8, 16), (32, 16), (16, 32), (64, 32), (32, 64),
+             (16, 12), (12, 16), (16, 4), (4, 16), (32, 24), (24, 32), (32, 8), (8, 32), (64, 48), (48, 64), (64, 16), (16, 64), (8, 4), (4, 8)]
+    for (w, h) in sizes:
+        for subme in (0, 3, 5):
+            merange = int(rng.integers(3, 12)) if method == 5 else (57 if method == 3 else 16)
+            r, o = _me_job(O, R, depth, rng, w, h, method, subme, 0, True, merange, qp=q)
+            assert G.R is None or r == o, (w, h, subme, r, o)
+            got.append(o); want.append(r)
+    assert len(got) == len(sizes) * 3
     G.same("results", lambda: want, got)
 
 

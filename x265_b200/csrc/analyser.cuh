@@ -165,6 +165,11 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     else if (p->subme < 0 || p->subme > 7) bad = "x265cu_analyser_create: subme outside 0..7";
     else if (p->width <= 0 || p->height <= 0 || (p->width & 7) || (p->height & 7))
         bad = "x265cu_analyser_create: width and height not positive multiples of 8";
+    // the quantiser's QPs: 0..51 + QP_BD_OFFSET (quant.cpp:224); k_cu_residual has scales for rem = qp % 6 in 0..5 only
+    else if (p->qp < 0 || p->qp > 51 + 6 * (p->depth - 8))
+        bad = "x265cu_analyser_create: qp outside 0..51 + 6 * (depth - 8)";
+    else if (!isfinite(p->lambda) || p->lambda < 0)
+        bad = "x265cu_analyser_create: lambda negative or not finite";
     if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return NULL; }
     cudaSetDevice(ctx->device);
     x265cu_analyser* a = new x265cu_analyser();
