@@ -1,5 +1,5 @@
 """GPU parity of the frame analyser with the chroma-SATD term of subpelCompare switched on (x265cu_analyser_enable_chroma:
-the ME stage runs the k_me_chroma launches on resident 4:2:0 planes) against the oracle's frame driver, which
+the ME stage runs the chroma instantiations of k_me on resident 4:2:0 planes) against the oracle's frame driver, which
 tests/test_frame_oracle_vs_ref.py::test_frame_driver_chroma pins to the real MotionEstimate (Yuv setSourcePU, bChroma).
 The kernels are the ones tests/test_gpu_me.py::test_me_batch_chroma covers; the analyser glue (plane residency, border
 extension, argument passing) first ran green on the round-1 driver box (GPUTEST_r01.json).  Kept in a file that sorts last so that a fault here cannot disturb the verified tests."""

@@ -283,7 +283,7 @@ int x265cu_analyser_load_inputs(x265cu_analyser* a, const void* fenc_host, int h
 }
 
 // ---- 4:2:0 chroma for the chroma-SATD term of subpelCompare (MotionEstimate::bChromaSATD, motion.cpp:204-212, 1601-1661) ----
-// After enable_chroma() the ME stage runs the k_me_chroma launches (x265cu_me_batch_chroma's kernels) on the resident chroma
+// After enable_chroma() the ME stage runs the chroma instantiations of k_me (x265cu_me_batch_chroma's kernels) on the resident chroma
 // planes; the caller uploads the source's Cb / Cr with load_chroma() and every reference's with set_ref_chroma().
 static int an_upload_cplane(x265cu_analyser* a, uint8_t* d_plane, const void* host, int hostStride)
 {

@@ -164,13 +164,8 @@ __global__ void __launch_bounds__(LA_WARPS * 32, 1) k_lookahead_cost(const x265c
             MeCtx<P> c;
             c.fenc = (const P*)jb.fenc[0] + off; c.fstride = stride; c.rstride = stride; c.mvc = mvcost;
             c.minx = mj.mvmin[0]; c.miny = mj.mvmin[1]; c.maxx = mj.mvmax[0]; c.maxy = mj.mvmax[1];
-            c.w = 8; c.h = 8; c.lgw = 3; c.lane = lane; c.lowres = 1; c.sm = sm; c.pow2 = true;
-            const int wpr = (8 * (int)sizeof(P)) >> 2;
-            c.lgwpr = 31 - __clz(wpr); c.nw = wpr * 8; c.lgnw = 31 - __clz(c.nw);
-            {
-                const unsigned fal = (unsigned)(uintptr_t)c.fenc | (unsigned)(stride * (int)sizeof(P));
-                c.lgsegw = min(c.lgwpr, (fal & 15u) == 0 ? 2 : (fal & 7u) == 0 ? 1 : 0);
-            }
+            c.w = 8; c.h = 8; c.lgw = 3; c.lane = lane; c.lowres = 1; c.sm = sm;
+            me_set_shape<P>(c);                 // source and reference share the stride
             int bcost = LA_COST_MAX, listused = 0;
             int lmx[2] = { 0, 0 }, lmy[2] = { 0, 0 };            // final MV of each list for the bidir candidates
             for (int i = 0; i < 1 + jb.bidir; i++)

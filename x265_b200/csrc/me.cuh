@@ -39,10 +39,31 @@ struct MeCtx
     MeShared* sm;
 };
 
-template <typename P>
-__device__ __forceinline__ int me_mvcost(const MeCtx<P>& c, int qx, int qy)
+// mvcost of the qpel vector (qx, qy) against the predictor (mvpx, mvpy): `mvc` is the centred table
+__device__ __forceinline__ int me_mvcost(const uint16_t* mvc, int mvpx, int mvpy, int qx, int qy)
 {
-    return (uint16_t)(__ldg(c.mvc + (qx - c.mvpx)) + __ldg(c.mvc + (qy - c.mvpy)));
+    return (uint16_t)(__ldg(mvc + (qx - mvpx)) + __ldg(mvc + (qy - mvpy)));
+}
+template <typename CTX>
+__device__ __forceinline__ int me_mvcost(const CTX& c, int qx, int qy) { return me_mvcost(c.mvc, c.mvpx, c.mvpy, qx, qy); }
+
+// PU shape fields of a search context (MeCtx or MeWin, which share the field names): whether w and h are powers of two,
+// words per row and per PU, and the widest lane segment (16 / 8 / 4 bytes) that both a PU row and the alignment of the
+// source block and its row pitch allow
+template <typename P> struct MeWin;                         // the shared-memory search window context (me_window.cuh)
+template <typename P>
+__device__ __forceinline__ unsigned me_fenc_align(const MeCtx<P>& c) { return (unsigned)(uintptr_t)c.fenc | (unsigned)(c.fstride * (int)sizeof(P)); }
+template <typename P>
+__device__ __forceinline__ unsigned me_fenc_align(const MeWin<P>& c) { return c.fenc | (unsigned)c.fpitch; }
+template <typename P, typename CTX>
+__device__ __forceinline__ void me_set_shape(CTX& c)
+{
+    c.pow2 = ((c.w & (c.w - 1)) | (c.h & (c.h - 1))) == 0;
+    const int wpr = (c.w * (int)sizeof(P)) >> 2;            // words per row (>= 1: w >= 4)
+    c.lgwpr = 31 - __clz(wpr);
+    c.nw = wpr * c.h; c.lgnw = 31 - __clz(c.nw);
+    const unsigned fal = me_fenc_align(c);
+    c.lgsegw = min(c.lgwpr, (fal & 15u) == 0 ? 2 : (fal & 7u) == 0 ? 1 : 0);
 }
 
 template <typename P>
@@ -156,19 +177,9 @@ __device__ __forceinline__ int me_sad_multi_t(const MeCtx<P>& c, const uint8_t* 
 template <typename P>
 __device__ __forceinline__ int me_sad_multi(const MeCtx<P>& c, const uint8_t* __restrict__ base, int n, int offB)
 {
-#ifdef ME_SEG_PER_BURST
-    // experiment (DESIGN.md section 8 item 1, build with -DME_SEG_PER_BURST): narrow the lane segment so that the lanes sharing a
-    // candidate fill one row before they spread over rows (fewer distinct lines per request for small-PU star bursts)
-    const int lgn = n <= 1 ? 0 : 32 - __clz(n - 1);
-    const int lgseg = min(c.lgsegw, max(0, c.lgwpr - (5 - lgn)));
-    if (lgseg == 2) return me_sad_multi_t<P, 2>(c, base, n, offB);
-    if (lgseg == 1) return me_sad_multi_t<P, 1>(c, base, n, offB);
-    return me_sad_multi_t<P, 0>(c, base, n, offB);
-#else
     if (c.lgsegw == 2) return me_sad_multi_t<P, 2>(c, base, n, offB);
     if (c.lgsegw == 1) return me_sad_multi_t<P, 1>(c, base, n, offB);
     return me_sad_multi_t<P, 0>(c, base, n, offB);
-#endif
 }
 
 // SAD of the fenc block against ONE reference position (element pointer, rows may be unaligned); all lanes get it.
@@ -628,11 +639,9 @@ __device__ __forceinline__ int me_subpel_multi_small(const MeCtx<P>& c, int n, i
     return c.w >= 8 ? me_subpel_small_t<P, 8>(c, n, qx, qy, satd) : me_subpel_small_t<P, 4>(c, n, qx, qy, satd);
 }
 
-// out-of-line copy for the cold multi-site users (pre-checks, lowres band cost)
+// out-of-line copy for the cold multi-site users (lowres pre-check candidates, AMP sizes)
 template <typename P>
 __device__ __noinline__ int me_subpel_compare(const MeCtx<P>& c, int qx, int qy, bool satd) { return me_subpel_compare_t(c, qx, qy, satd); }
-template <typename P>
-__device__ __noinline__ int me_band_cost_ni(const MeCtx<P>& c, int y0, int rows, bool satd) { return me_band_cost(c, y0, rows, satd); }
 
 // PU classes of the sub-pel stage: 0 = small (pow2, w and h <= 16: four candidates at a time through
 // me_subpel_multi_small), 1 = everything else (one candidate at a time, banded).  CLS = -1 compiles both.
@@ -665,32 +674,6 @@ __device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx,
         }
     }
     return out;
-}
-
-// lowresQPelCost (lowres.h:94-120): qpel = rounded average of the two nearest hpel planes; 8x8 blocks
-template <typename P>
-__device__ __noinline__ int me_lowres_cost(const MeCtx<P>& c, int qx, int qy, bool satd)
-{
-    if ((qx | qy) & 1)
-    {
-        int ha = (qy & 2) | ((qx & 2) >> 1);
-        const P* a = c.ref[ha] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride;
-        int rx = qx + (qx & 1), ry = qy + (qy & 1);
-        int hb = (ry & 2) | ((rx & 2) >> 1);
-        const P* b = c.ref[hb] + (rx >> 2) + (ptrdiff_t)(ry >> 2) * c.rstride;
-        __syncwarp();
-        for (int i = c.lane; i < 64; i += 32)
-        {
-            int y = i >> 3, x = i & 7;
-            c.sm->pred[y * 64 + x] = (uint16_t)(((int)a[(ptrdiff_t)y * c.rstride + x] + (int)b[(ptrdiff_t)y * c.rstride + x] + 1) >> 1);
-        }
-        __syncwarp();
-        return warp_sum(me_band_cost_ni(c, 0, c.h, satd));
-    }
-    int hp = (qy & 2) | ((qx & 2) >> 1);
-    const P* r = c.ref[hp] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride;
-    if (!satd) return me_sad_direct(c, r);
-    return warp_satd(c.fenc, c.fstride, r, c.rstride, c.w, c.h, c.lane);
 }
 
 // SATD partial of one row segment: horizontal 4-point Hadamards in registers, vertical ones over the 4 lanes of a
@@ -743,7 +726,7 @@ __device__ __forceinline__ void me_load_row8(const P* __restrict__ p, int (&v)[8
 // lowresQPelCost (lowres.h:94-120) of up to 4 candidates of an 8x8 lowres CU at once: 8 lanes per candidate, one
 // row each; the row of the prediction (one half-pel plane, or the rounded average of the two nearest for odd
 // quarter-pel positions) stays in registers, SATD = two 8x4 tiles through the shuffle butterflies.  Lane i (< n)
-// gets candidate i's distortion.  Same arithmetic as me_lowres_cost.
+// gets candidate i's distortion.
 template <typename P>
 __device__ __forceinline__ int me_lowres_multi(const MeCtx<P>& c, int n, int qx, int qy, bool satd)
 {
@@ -800,22 +783,9 @@ __device__ __forceinline__ int me_lowres_batch(const MeCtx<P>& c, int n, int qx,
     return out;
 }
 
-template <typename P>
-__device__ __forceinline__ int me_qpel_cost(const MeCtx<P>& c, int qx, int qy, bool satd)
-{
-    return c.lowres ? me_lowres_cost(c, qx, qy, satd) : me_subpel_compare(c, qx, qy, satd);
-}
-
-template <typename P>
-__device__ __forceinline__ int me_cost_fpel(const MeCtx<P>& c, int x, int y)
-{
-    return me_sad_direct(c, c.ref[0] + x + (ptrdiff_t)y * c.rstride) + me_mvcost(c, x * 4, y * 4);
-}
-
 struct MeStar { int bx, by, bcost, point, dist; };
 
 // shared-memory search window context (me_window.cuh): its evaluation sites are overloads of the same names
-template <typename P> struct MeWin;
 template <typename P> __device__ __forceinline__ int me_eval_points(const MeWin<P>& c, int n, int px, int py, bool x8);
 template <typename P> __device__ __forceinline__ void me_raster(const MeWin<P>& c, MeStar& s);
 
@@ -1657,36 +1627,27 @@ __device__ __forceinline__ void me_make_ctx(MeCtx<P>& c, const x265cu_me_job& j,
     c.mvpx = j.qmvp[0]; c.mvpy = j.qmvp[1];
     c.minx = j.mvmin[0]; c.miny = j.mvmin[1]; c.maxx = j.mvmax[0]; c.maxy = j.mvmax[1];
     c.w = j.pw; c.h = j.ph; c.lgw = 31 - __clz(c.w); c.lane = lane; c.lowres = lowres; c.sm = sm;
-    c.pow2 = ((c.w & (c.w - 1)) | (c.h & (c.h - 1))) == 0;
-    const int wpr = (c.w * (int)sizeof(P)) >> 2;            // words per row (>= 1: w >= 4)
-    c.lgwpr = 31 - __clz(wpr);
-    c.nw = wpr * c.h; c.lgnw = 31 - __clz(c.nw);
-    // widest lane segment (16 / 8 / 4 bytes) that both a PU row and the fenc row alignment allow
-    const unsigned fal = (unsigned)(uintptr_t)c.fenc | (unsigned)(fstride * (int)sizeof(P));
-    c.lgsegw = min(c.lgwpr, (fal & 15u) == 0 ? 2 : (fal & 7u) == 0 ? 1 : 0);
+    me_set_shape<P>(c);
     if ((unsigned)(rstride * (int)sizeof(P)) & 7u) c.lgsegw = 0;        // the 8-byte aligned reference loads need an 8-byte row pitch
 }
 
 // Persistent warps with a dynamic job queue (jobs differ by up to 64x in work).  The search is split into
 // launches -- pre-checks (small PUs, other PUs), integer search, sub-pel refinement (small PUs, other PUs) --
 // because the fused body (12.4 K SASS instructions, ~200 KB) thrashes the instruction cache, and so does an
-// un-split sub-pel kernel (8.8 K instructions, both PU classes resident on every SM).  PHASE 0 = all fused
-// (the lookahead kernel's per-CU call).
-#ifndef ME_MIN_BLOCKS
-#define ME_MIN_BLOCKS 3
-#endif
-#ifndef ME_P2_BLOCKS
-#define ME_P2_BLOCKS 4
-#endif
-#ifndef ME_BIG_BLOCKS
-#define ME_BIG_BLOCKS 2          // large-PU pre-check / sub-pel kernels: 128 registers beat a third resident CTA (no spills in the tap loops)
-#endif
-template <typename P, int PHASE, int CLS>
+// un-split sub-pel kernel (8.8 K instructions, both PU classes resident on every SM).  The lookahead kernel runs
+// the fused body per CU (me_run_job).
+// CTAs per SM: integer search, small-PU pre-check / sub-pel kernels, and the large-PU ones, where 128 registers beat a
+// third resident CTA (no spills in the tap loops)
+constexpr int ME_P2_BLOCKS = 4, ME_MIN_BLOCKS = 3, ME_BIG_BLOCKS = 2;
+// CHROMA: the pre-check and sub-pel launches with the chroma-SATD term (x265cu_me_batch_chroma), separate instantiations so
+// that the luma-only kernels carry no chroma code.  They run full-resolution planes only (the lowres planes have no
+// chroma), and the integer search (phase 2) is luma only in the reference too.
+template <typename P, int PHASE, int CLS, bool CHROMA>
 __global__ void __launch_bounds__(256, PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS)) k_me(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, int lowres,
-                                                           const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs, int n,
+                                                           MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs, int n,
                                                            int32_t* __restrict__ out, MeState* __restrict__ state, int* __restrict__ counter,
-                                                           const int32_t* __restrict__ list = nullptr, const int* __restrict__ list_n = nullptr,
-                                                           const int32_t* __restrict__ order = nullptr, int order0 = 0)
+                                                           const int32_t* __restrict__ list, const int* __restrict__ list_n,
+                                                           const int32_t* __restrict__ order, int order0)
 {
     extern __shared__ unsigned char me_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1705,82 +1666,34 @@ __global__ void __launch_bounds__(256, PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? M
         if (order) jid = order[jid] - order0;
         const x265cu_me_job j = jobs[jid];
         MeCtx<P> c;
-        me_make_ctx<P>(c, j, fenc, fstride, refs, rstride, lowres, mvcost, lane, sm);
+        me_make_ctx<P>(c, j, fenc, fstride, refs, rstride, CHROMA ? 0 : lowres, mvcost, lane, sm);
         if (CLS >= 0 && me_subpel_class(c) != CLS) continue;                   // the sibling launch owns this job
-        if (PHASE == 0) me_run_job<P>(c, j, out + (size_t)jid * 4);
-        else
-        {
-            MeState st;
-            if (PHASE != 1) st = state[jid];
-            if (PHASE == 1) { me_phase1<P, CLS>(c, j, st); if (lane == 0) state[jid] = st; }
-            if (PHASE == 2) { me_phase2<P>(c, j, st); if (lane == 0) state[jid] = st; }
-            if (PHASE == 3) me_phase3<P, CLS>(c, j, st, out + (size_t)jid * 4);
-        }
-        __syncwarp();
-    }
-}
-
-// The pre-check and sub-pel launches with the chroma-SATD term (x265cu_me_batch_chroma): separate instantiations, so
-// the luma-only kernels above are unchanged by it.  The integer search (phase 2) is luma only in the reference too.
-template <typename P, int PHASE, int CLS>
-__global__ void __launch_bounds__(256, CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS) k_me_chroma(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride,
-                                                           MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs, int n,
-                                                           int32_t* __restrict__ out, MeState* __restrict__ state, int* __restrict__ counter,
-                                                           const int32_t* __restrict__ list = nullptr, const int* __restrict__ list_n = nullptr,
-                                                           const int32_t* __restrict__ order = nullptr, int order0 = 0)
-{
-    extern __shared__ unsigned char me_smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    MeShared* sm = (MeShared*)me_smem + warp;
-    if (list) n = *list_n;                             // the jobs list[0 .. *list_n) (see k_me)
-    for (;;)
-    {
-        int jid = 0;
-        if (lane == 0) jid = atomicAdd(counter, 1);
-        jid = __shfl_sync(0xffffffffu, jid, 0);
-        if (jid >= n) break;
-        if (list) jid = list[jid];
-        if (order) jid = order[jid] - order0;          // shape-sorted job order (see k_me)
-        const x265cu_me_job j = jobs[jid];
-        MeCtx<P> c;
-        me_make_ctx<P>(c, j, fenc, fstride, refs, rstride, 0, mvcost, lane, sm);
-        if (me_subpel_class(c) != CLS) continue;                   // the sibling launch owns this job
         MeChromaCtx<P> cc;
-        me_set_chroma<P>(cc, c, j, ch, fstride);
+        if (CHROMA) me_set_chroma<P>(cc, c, j, ch, fstride);
         MeState st;
-        if (PHASE == 1) { me_phase1<P, CLS, true>(c, j, st, &cc); if (lane == 0) state[jid] = st; }
-        else            { st = state[jid]; me_phase3<P, CLS, true>(c, j, st, out + (size_t)jid * 4, &cc); }
+        if (PHASE != 1) st = state[jid];
+        if (PHASE == 1) { me_phase1<P, CLS, CHROMA>(c, j, st, &cc); if (lane == 0) state[jid] = st; }
+        if (PHASE == 2) { me_phase2<P>(c, j, st); if (lane == 0) state[jid] = st; }
+        if (PHASE == 3) me_phase3<P, CLS, CHROMA>(c, j, st, out + (size_t)jid * 4, &cc);
         __syncwarp();
     }
 }
 
+// One launch of k_me; `ch` != NULL selects the chroma instantiation (pre-check and sub-pel phases only)
 template <typename P, int PHASE, int CLS>
-static int launch_me_chroma_phase(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs& ch,
-                                  const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, MeState* state, int* counter,
-                                  const int32_t* list = NULL, const int* list_n = NULL, const int32_t* order = NULL, int order0 = 0)
-{
-    const int threads = 256, warps = threads / 32;
-    const size_t smem = sizeof(MeShared) * warps;
-    int blocks = ctx->sm_count * (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS);
-    int need = (n + warps - 1) / warps;
-    if (blocks > need) blocks = need;
-    k_me_chroma<P, PHASE, CLS><<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ch, mvcost, jobs, n, out, state, counter,
-                                                                       list, list_n, order, order0);
-    CU_LAUNCH_CHECK(ctx);
-    return 0;
-}
-
-template <typename P, int PHASE, int CLS>
-static int launch_me_phase(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres,
+static int launch_me_phase(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres, const MeChromaArgs* ch,
                            const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, MeState* state, int* counter,
-                           const int32_t* list = NULL, const int* list_n = NULL, const int32_t* order = NULL, int order0 = 0)
+                           const int32_t* list, const int* list_n, const int32_t* order, int order0)
 {
     const int threads = 256, warps = threads / 32;
     const size_t smem = PHASE == 2 ? 0 : sizeof(MeShared) * warps;      // the integer search never touches the interpolation scratch
     int blocks = ctx->sm_count * (PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS));
     int need = (n + warps - 1) / warps;
     if (blocks > need) blocks = need;
-    k_me<P, PHASE, CLS><<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, lowres, mvcost, jobs, n, out, state, counter, list, list_n, order, order0);
+    const MeChromaArgs none = {};
+    const auto kernel = ch ? k_me<P, PHASE, CLS, PHASE != 2> : k_me<P, PHASE, CLS, false>;
+    kernel<<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, lowres, ch ? *ch : none, mvcost, jobs, n, out,
+                                                   state, counter, list, list_n, order, order0);
     CU_LAUNCH_CHECK(ctx);
     return 0;
 }
@@ -1809,52 +1722,26 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
                        const MeChromaArgs* ch, const MeWinLaunch* win)
 {
     int rc = 0;
-    // shape-sorted job order (geometry.h `order`): it helps kernels that miss the instruction cache (the chroma sub-pel
-    // launches) and slows the others (they lose the raster order's L1 / L2 locality).  X265CU_ME_ORDER = 0: never, 1: chroma sub-pel launches
-    // only (default), 2: every pre-check / sub-pel launch.
-    static const int ordMode = [] { const char* e = getenv("X265CU_ME_ORDER"); return e ? atoi(e) : 1; }();
-    const int32_t* ordAll = (win && !lowres) ? win->order : NULL;
-    const int32_t* ord = ordMode >= 2 ? ordAll : NULL;                       // pre-checks, luma-only sub-pel
-    const int32_t* ord3 = (ordMode >= 2 || (ordMode == 1 && ch)) ? ordAll : NULL;   // chroma sub-pel
+    // with job groups (the frame analyser), the pre-checks of the 16x16 cells come out of shared per-cell tables
+    // (me_window.cuh) and the integer search of the STAR groups out of shared-memory windows; the per-PU kernels then run
+    // only the jobs listed in the window search's leftover list, which is free until the integer search
+    const bool grp = win && !lowres;
+    const int32_t* left = grp ? win->left_list : NULL;
+    const int* left_n = grp ? win->left_count : NULL;
+    // shape-sorted job order (geometry.h `order`) for the chroma sub-pel launches: it helps kernels that miss the instruction
+    // cache and slows the others (they lose the raster order's L1 / L2 locality)
+    const int32_t* ord = ch && grp ? win->order : NULL;
     const int ord0 = win ? win->job0 : 0;
-    // pre-checks: with job groups, the 16x16 cells out of shared per-cell tables (me_window.cuh) and only the other jobs
-    // through the per-PU kernels; the window search's leftover list is free until the integer search and carries them
-    const int32_t* pre = NULL; const int* pre_n = NULL; const int32_t* ord1 = ord;
-    if (win && !lowres)
-    {
-        rc |= launch_me_precheck_groups<P>(ctx, fenc, fstride, refs, rstride, ch, mvcost, jobs, st, *win, win->left_count, win->left_list);
-        pre = win->left_list; pre_n = win->left_count; ord1 = NULL;
-    }
-    if (ch)
-    {
-        rc |= launch_me_chroma_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 0, pre, pre_n, ord1, ord0);
-        rc |= launch_me_chroma_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 1, pre, pre_n, ord1, ord0);
-    }
-    else
-    {
-        rc |= launch_me_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 0, pre, pre_n, ord1, ord0);
-        rc |= launch_me_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 1, pre, pre_n, ord1, ord0);
-    }
+    if (grp) rc |= launch_me_precheck_groups<P>(ctx, fenc, fstride, refs, rstride, ch, mvcost, jobs, st, *win, win->left_count, win->left_list);
+    rc |= launch_me_phase<P, 1, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 0, left, left_n, NULL, 0);
+    rc |= launch_me_phase<P, 1, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 1, left, left_n, NULL, 0);
     CU_CHECK(cudaEventRecord(ctx->me_ev[1], ctx->stream));
-    if (win && !lowres)
-    {
-        // STAR groups out of shared-memory windows; whatever does not fit (or is not STAR) through the global-memory kernel
-        rc |= launch_me_window<P>(ctx, fenc, fstride, mvcost, jobs, st, *win);
-        rc |= launch_me_phase<P, 2, -1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 2, win->left_list, win->left_count);
-    }
-    else
-        rc |= launch_me_phase<P, 2, -1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 2);
+    // STAR groups out of shared-memory windows; whatever does not fit (or is not STAR) through the global-memory kernel
+    if (grp) rc |= launch_me_window<P>(ctx, fenc, fstride, mvcost, jobs, st, *win);
+    rc |= launch_me_phase<P, 2, -1>(ctx, fenc, fstride, refs, rstride, lowres, NULL, mvcost, jobs, n, out, st, counter_dev + 2, left, left_n, NULL, 0);
     CU_CHECK(cudaEventRecord(ctx->me_ev[2], ctx->stream));
-    if (ch)
-    {
-        rc |= launch_me_chroma_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord3, ord0);
-        rc |= launch_me_chroma_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, *ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord3, ord0);
-    }
-    else
-    {
-        rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0);
-        rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0);
-    }
+    rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0);
+    rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0);
     return rc;
 }
 

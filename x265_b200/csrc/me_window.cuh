@@ -18,7 +18,7 @@
 //        (candidate, row, 16 bytes): one broadcast LDS.128 + four VABSDIFF4, the reference row is fetched once per
 //        ceil(h / 5) candidates.  Costs, ties and the `mvcost(tmv << 3)` quirk of every 4th column are the reference's.
 // Groups whose union window does not fit the shared-memory budget, or that are not STAR jobs, are appended to a leftover
-// list that the global-memory kernel (k_me<P,2,-1>) drains afterwards: same results, no CPU or library fallback.
+// list that the global-memory kernel (k_me<P, 2, -1, false>) drains afterwards: same results, no CPU or library fallback.
 #pragma once
 #include "common.cuh"
 #include "me.cuh"
@@ -89,12 +89,6 @@ __device__ __forceinline__ uint2 lds64(uint32_t a) { uint2 v; asm volatile("ld.s
 __device__ __forceinline__ uint32_t lds16(uint32_t a) { uint32_t v; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ void sts16(uint32_t a, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ uint4 lds128(uint32_t a) { uint4 v; asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; }
-
-template <typename P>
-__device__ __forceinline__ int mew_mvcost(const MeWin<P>& c, int qx, int qy)
-{
-    return (uint16_t)(__ldg(c.mvc + (qx - c.mvpx)) + __ldg(c.mvc + (qy - c.mvpy)));
-}
 
 // SEGW words of a window row starting at a byte address of any phase: SEGW + 1 aligned LDS.32 + SEGW funnel shifts.
 // (The global-memory core reads 8-byte aligned LDG.64 pairs and selects: fewer load instructions matter on the L1 path.  Out
@@ -196,7 +190,7 @@ __device__ __forceinline__ int me_eval_points(const MeWin<P>& c, int n, int px, 
         }
     }
     int cost = 0x7fffffff;
-    if (c.lane < n) cost = mysad + (x8 ? mew_mvcost(c, px * 8, py * 8) : mew_mvcost(c, px * 4, py * 4));
+    if (c.lane < n) cost = mysad + (x8 ? me_mvcost(c, px * 8, py * 8) : me_mvcost(c, px * 4, py * 4));
     return cost;
 }
 // ---- raster refinement out of the window (motion.cpp:1171-1201) ---------------------------------------------------
@@ -529,7 +523,7 @@ __device__ __forceinline__ int me_star_lookup(const MeWinCell<P>& c, int mylvl, 
         sad += (int)(((e >= 2 ? v.y : v.x) >> ((e & 1) * 16)) & 0xffffu);
         if (sx >= 0) sad -= (int)(((sx >= 2 ? v.y : v.x) >> ((sx & 1) * 16)) & 0xffffu);
     }
-    return sad + mew_mvcost(c, px * 4, py * 4);
+    return sad + me_mvcost(c, px * 4, py * 4);
 }
 
 // Star table of a cell: thread = (candidate, block row); 4 rows of the cell against the window at the candidate's vector.
@@ -761,11 +755,7 @@ __global__ void __launch_bounds__(256, 3) k_me_window(const P* __restrict__ fenc
         c.mvc = mvcost; c.mvpx = j.qmvp[0]; c.mvpy = j.qmvp[1];
         c.minx = j.mvmin[0]; c.miny = j.mvmin[1]; c.maxx = j.mvmax[0]; c.maxy = j.mvmax[1];
         c.w = j.pw; c.h = j.ph; c.lane = lane;
-        c.pow2 = ((c.w & (c.w - 1)) | (c.h & (c.h - 1))) == 0;
-        const int wpr = (c.w * ES) >> 2;
-        c.lgwpr = 31 - __clz(wpr); c.nw = wpr * c.h; c.lgnw = 31 - __clz(c.nw);
-        const unsigned fal = c.fenc | (unsigned)c.fpitch;
-        c.lgsegw = min(c.lgwpr, (fal & 15u) == 0 ? 2 : (fal & 7u) == 0 ? 1 : 0);
+        me_set_shape<P>(c);                                        // the window's pitch is a multiple of 16 bytes
         c.cell = NULL;
         if (CELL && hdr->cell.on && c.minx == hdr->cell.minx && c.maxx == hdr->cell.maxx && c.miny == hdr->cell.miny && c.maxy == hdr->cell.maxy)
             c.cell = &hdr->cell;
@@ -841,18 +831,10 @@ static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, cons
         MeWinArgs a;
         a.tmaps = (const CUtensorMap*)w.tmaps; a.allocX = w.allocX; a.allocY = w.allocY;
         a.smemBytes = mew_smem_bytes((int)sizeof(P), cls, &a.fencBytes);
-        if (cls < 2)
-        {
-            CU_CHECK(cudaFuncSetAttribute(k_me_window<P, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smemBytes));
-            k_me_window<P, false><<<w.ngroups[cls], threads, a.smemBytes, ctx->stream>>>((const P*)fenc, fstride, a, mvcost, jobs, (const MeGroup*)w.groups[cls],
-                                                                                    w.grp_jobs[cls], w.job0, st, w.left_count, w.left_list);
-        }
-        else
-        {
-            CU_CHECK(cudaFuncSetAttribute(k_me_window<P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smemBytes));
-            k_me_window<P, true><<<w.ngroups[cls], threads, a.smemBytes, ctx->stream>>>((const P*)fenc, fstride, a, mvcost, jobs, (const MeGroup*)w.groups[cls],
-                                                                                   w.grp_jobs[cls], w.job0, st, w.left_count, w.left_list);
-        }
+        const auto kernel = cls == 2 ? k_me_window<P, true> : k_me_window<P, false>;
+        CU_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, a.smemBytes));
+        kernel<<<w.ngroups[cls], threads, a.smemBytes, ctx->stream>>>((const P*)fenc, fstride, a, mvcost, jobs, (const MeGroup*)w.groups[cls],
+                                                                      w.grp_jobs[cls], w.job0, st, w.left_count, w.left_list);
         CU_LAUNCH_CHECK(ctx);
     }
     return 0;
@@ -1033,21 +1015,21 @@ __global__ void __launch_bounds__(256) k_me_precheck_cell(const P* __restrict__ 
         // me_phase1's fold
         const int mvpx = j.qmvp[0], mvpy = j.qmvp[1];
         int bprecost = L[0] + C[0], bcost = bprecost, bestprex = pmvx, bestprey = pmvy, jbmx = bmx, jbmy = bmy;
-        if (frac) bcost = L[1] + (uint16_t)(__ldg(mvcost + (bmx * 4 - mvpx)) + __ldg(mvcost + (bmy * 4 - mvpy)));
+        if (frac) bcost = L[1] + me_mvcost(mvcost, mvpx, mvpy, bmx * 4, bmy * 4);
         if (nonzero)
         {
-            const int cz = L[2] + (uint16_t)(__ldg(mvcost - mvpx) + __ldg(mvcost - mvpy));
+            const int cz = L[2] + me_mvcost(mvcost, mvpx, mvpy, 0, 0);
             if (cz < bcost) { bcost = cz; jbmx = 0; jbmy = max(min(0, (int)j.mvmax[1]), (int)j.mvmin[1]); }
         }
         int cbest = 0x7fffffff, cbx = 0, cby = 0;
         if (v0)
         {
-            const int cost = L[3] + C[1] + (uint16_t)(__ldg(mvcost + (c0x - mvpx)) + __ldg(mvcost + (c0y - mvpy)));
+            const int cost = L[3] + C[1] + me_mvcost(mvcost, mvpx, mvpy, c0x, c0y);
             cbest = cost; cbx = c0x; cby = c0y;
         }
         if (v1)
         {
-            const int cost = L[4] + C[2] + (uint16_t)(__ldg(mvcost + (c1x - mvpx)) + __ldg(mvcost + (c1y - mvpy)));
+            const int cost = L[4] + C[2] + me_mvcost(mvcost, mvpx, mvpy, c1x, c1y);
             if (cost < cbest) { cbest = cost; cbx = c1x; cby = c1y; }
         }
         if (cbest < bprecost) { bprecost = cbest; bestprex = cbx; bestprey = cby; }
@@ -1069,10 +1051,9 @@ static int launch_me_precheck_groups(x265cu_ctx* ctx, const void* fenc, int fstr
     {
         if (w.ngroups[cls] <= 0) continue;
         const int blocks = (w.ngroups[cls] + 7) / 8;
-        if (ch) k_me_precheck_cell<P, true><<<blocks, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, *ch, mvcost, jobs,
-                                                                            (const MeGroup*)w.groups[cls], w.ngroups[cls], w.grp_jobs[cls], w.job0, cls == 2, st, left_count, left_list);
-        else    k_me_precheck_cell<P, false><<<blocks, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, none, mvcost, jobs,
-                                                                             (const MeGroup*)w.groups[cls], w.ngroups[cls], w.grp_jobs[cls], w.job0, cls == 2, st, left_count, left_list);
+        const auto kernel = ch ? k_me_precheck_cell<P, true> : k_me_precheck_cell<P, false>;
+        kernel<<<blocks, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ch ? *ch : none, mvcost, jobs,
+                                                (const MeGroup*)w.groups[cls], w.ngroups[cls], w.grp_jobs[cls], w.job0, cls == 2, st, left_count, left_list);
         CU_LAUNCH_CHECK(ctx);
     }
     return 0;

@@ -315,9 +315,8 @@ static int launch_transform_mma(x265cu_ctx* ctx, int op, int N, const int16_t* s
     }
     int blocks = (n + 7) / 8;
     if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-    // inverse: role-swapped pass 2 with 4-byte stores when every destination row is 4-byte aligned (X265CU_IDCT_SWAP=0 disables)
-    static const int swapOn = [] { const char* e = getenv("X265CU_IDCT_SWAP"); return e ? atoi(e) : 1; }();
-    const int vec = swapOn && !fwd && !(((uintptr_t)dst) & 3) && !(stride & 1) && !(tu_pitch & 1);
+    // inverse: role-swapped pass 2 with 4-byte stores when every destination row is 4-byte aligned
+    const int vec = !fwd && !(((uintptr_t)dst) & 3) && !(stride & 1) && !(tu_pitch & 1);
     if (N == 32)
     {
         if (fwd) k_transform_mma<DEPTH, 32, true><<<blocks, 256, 0, ctx->stream>>>(src, dst, stride, tu_pitch, n, 0);
