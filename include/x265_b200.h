@@ -247,7 +247,12 @@ int x265cu_analyser_analyse(x265cu_analyser*, const void* fenc_host, int host_st
 int x265cu_analyser_stage_ms(x265cu_analyser*, float ms[4]);          /* device ms of the last run: ME stage, residual, intra, ME kernel */
 void* x265cu_analyser_ref_plane(x265cu_analyser*, int idx, int* stride); /* device address of ref idx's pixel (0,0) */
 int x265cu_analyser_ref_updated(x265cu_analyser*, int idx);            /* re-extend borders after writing the plane in place */
-int x265cu_analyser_fetch(x265cu_analyser*, int what, void* host);    /* parity/debug access to resident results */
+int x265cu_analyser_fetch(x265cu_analyser*, int what, void* host);    /* parity/debug access to resident results; what =
+                                                                          16 + 16 * ref + yf * 4 + xf: the whole allocation of
+                                                                          reference ref's quarter-pel phase plane (xf, yf) */
+/* Every reference of an analyser is stored with its 15 quarter-pel phase planes, which every ME run rebuilds for the
+ * sub-pel refinement: 15 planes of (width + 192, 64-aligned) x (height + 160) pixels per reference, e.g. 561 MB at
+ * 3840x2160 8-bit with 4 references, 1.40 GB at 3840x2160 10-bit with 5, 5.3 GB at 7680x4320 10-bit with 5. */
 /* CTU-row shards (BASELINE configs[4]: WPP CTU rows sharded per GPU; the reference enables row r once the reference
  * rows it needs are reconstructed, frameencoder.cpp:850-868, producer side framefilter.cpp:664).  All job / CU / TU
  * lists are in CTU raster order, so rows [ctuRow0, ctuRow1) are one contiguous slice of every result array

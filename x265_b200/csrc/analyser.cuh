@@ -6,6 +6,7 @@
 #include "me.cuh"
 #include "me_window.cuh"
 #include <vector>
+#include <climits>
 #include <stdlib.h>
 
 struct x265cu_analyser
@@ -39,6 +40,11 @@ struct x265cu_analyser
     int windowOn; MeGroup* d_groups[3]; int32_t* d_grpJobs[3]; std::vector<int> rowGrp[3];
     CUtensorMap* d_tmaps; int32_t* d_left;
     int32_t* d_order;                     // jobs of every CTU row sorted by PU shape (geometry.h)
+    // quarter-pel phase planes of the sub-pel refinement (MePlanes, me.cuh): d_refs[r] is a block of 16 planes planeBytes
+    // apart, slot 0 = the reference plane, slot yf * 4 + xf = phase (xf, yf); tile jobs of their build (hpp / vpp / hvpp
+    // phases, the same for every reference); per CTU row, the rectangle its sub-pel launches can read (AnRect below)
+    x265cu_interp_job* d_planeJobs[3]; int nPlaneJobs[3];
+    std::vector<int4> rowRead;
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -68,6 +74,84 @@ static void an_build_geometry(x265cu_analyser* a)
     }
 }
 
+// ---- phase planes: what the sub-pel launches read and what the build writes ----
+// Rectangles are picture-relative pixel coordinates of a phase plane, x0..x1 and y0..y1 inclusive.
+// READ, per PU: k_build_me_jobs clips the search range to full-pel vectors in [-(71 + cuX), width + 7 - cuX] x
+// [-(71 + cuY), height + 7 - cuY] (clipMv, cudata.cpp:1915-1928).  y: me_phase3 keeps every sub-pel candidate inside
+// [qminy, qmaxy], its centre is the search winner (in range, or MV 0), so the block's rows are the PU's rows moved by
+// [-(71 + cuY), height + 7 - cuY].  x is not range-checked: the HEX search ends up to 3 full pels outside [minx, maxx]
+// (DIA 1, STAR and FULL 0, or at MV 0), then the sub-pel rounds move up to 6 quarter pels (2 half-pel + 2 quarter-pel
+// iterations at subme 7), so the block's full-pel column lies in [minx - 5, maxx + 4].
+// BUILT: columns [-AN_PLANE_X, width + AN_PLANE_X), rows [-AN_PLANE_Y, height + AN_PLANE_Y).  The 8-tap support of a built
+// pixel (3 before, 4 after) and the aligned-word over-read of the row filter (up to 8 bytes past it) stay inside the margins.
+// The clip does not depend on where the CU is, so the PUs of any CTU row can reach rows -71 .. height + 70: every run
+// builds the whole rectangle, whatever rows it analyses.  Pixels outside BUILT stay 0 (zeroed at allocation) and are only
+// ever loaded as the unused bytes of an aligned word.
+static const int AN_PLANE_X = 80, AN_PLANE_Y = 76, AN_PLANE_TILE = 64;
+
+static int4 an_rect_union(int4 a, int4 b) { return make_int4(min(a.x, b.x), min(a.y, b.y), max(a.z, b.z), max(a.w, b.w)); }
+
+// READ of the PUs of every CTU row, (x0, y0, x1, y1)
+static void an_build_read_rects(x265cu_analyser* a)
+{
+    const int W = a->p.width, H = a->p.height;
+    a->rowRead.assign(a->ctuRows, make_int4(INT_MAX, INT_MAX, INT_MIN, INT_MIN));
+    for (int r = 0; r < a->ctuRows; r++)
+        for (int i = a->rowJob[r]; i < a->rowJob[r + 1]; i++)
+        {
+            const PuDesc& d = a->pus[i];
+            const int y = d.offset / a->stride, x = d.offset - y * a->stride;
+            a->rowRead[r] = an_rect_union(a->rowRead[r], make_int4(x - (71 + d.cuX) - 5, y - (71 + d.cuY),
+                                                                   x + d.pw - 1 + (W + 7 - d.cuX) + 4, y + d.ph - 1 + (H + 7 - d.cuY)));
+        }
+}
+
+// BUILT contains READ of the CTU rows [r0, r1), and BUILT's filter support lies inside the plane allocation
+static bool an_planes_cover(const x265cu_analyser* a, int r0, int r1)
+{
+    const int W = a->p.width, H = a->p.height;
+    int4 rd = make_int4(INT_MAX, INT_MAX, INT_MIN, INT_MIN);
+    for (int r = r0; r < r1; r++) rd = an_rect_union(rd, a->rowRead[r]);
+    const bool covers = rd.x >= -AN_PLANE_X && rd.y >= -AN_PLANE_Y && rd.z < W + AN_PLANE_X && rd.w < H + AN_PLANE_Y;
+    const int es = a->p.depth == 8 ? 1 : 2;
+    const bool inside = -AN_PLANE_X - 3 >= -AN_MARGIN_X && -AN_PLANE_Y - 3 >= -AN_MARGIN_Y &&
+                        (W + AN_PLANE_X + 4) * es + 8 <= (a->stride - AN_MARGIN_X) * es && H + AN_PLANE_Y + 4 <= H + AN_MARGIN_Y;
+    return covers && inside;
+}
+
+// tile jobs of the build over BUILT, relative to a reference's block base: hpp (xf = 1..3), vpp (yf = 1..3), hvpp (both)
+static int an_build_plane_jobs(x265cu_analyser* a)
+{
+    const size_t es = a->p.depth == 8 ? 1 : 2;
+    const int64_t ppitch = (int64_t)(a->planeBytes / es), org = (int64_t)(a->orgBytes / es);
+    const int X1 = a->p.width + AN_PLANE_X, Y1 = a->p.height + AN_PLANE_Y;
+    for (int g = 0; g < 3; g++)
+    {
+        std::vector<x265cu_interp_job> jobs;
+        for (int yf = 0; yf < 4; yf++)
+            for (int xf = 0; xf < 4; xf++)
+            {
+                if ((g == 0 && (!xf || yf)) || (g == 1 && (xf || !yf)) || (g == 2 && (!xf || !yf))) continue;
+                for (int y = -AN_PLANE_Y; y < Y1; y += AN_PLANE_TILE)
+                    for (int x = -AN_PLANE_X; x < X1; x += AN_PLANE_TILE)
+                    {
+                        x265cu_interp_job j = {};
+                        j.s_off = org + (int64_t)y * a->stride + x;
+                        j.d_off = (yf * 4 + xf) * ppitch + j.s_off;
+                        j.s_stride = j.d_stride = a->stride;
+                        j.w = (int16_t)min(AN_PLANE_TILE, X1 - x); j.h = (int16_t)min(AN_PLANE_TILE, Y1 - y);
+                        j.idxX = (int8_t)(g == 1 ? yf : xf); j.idxY = (int8_t)yf;          // the vertical filters take idxX
+                        j.ntaps = 8;
+                        jobs.push_back(j);
+                    }
+            }
+        a->nPlaneJobs[g] = (int)jobs.size();
+        a->d_planeJobs[g] = an_upload(a->ctx, jobs);
+        if (!a->d_planeJobs[g]) return -1;
+    }
+    return 0;
+}
+
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
 // the intra table are indexed by the slice-local index inside the kernels, CU / TU records carry absolute indices.
 static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
@@ -76,6 +160,11 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     const int depth = a->p.depth;
     cudaSetDevice(c->device);
     if (r0 < 0 || r1 > a->ctuRows || r0 >= r1) { x265cu_set_error("analyser: bad CTU row range", cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    if ((stages & 1) && !an_planes_cover(a, r0, r1))
+    {
+        x265cu_set_error("analyser: the phase planes do not cover the rows the sub-pel search can read", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
     const int tu0 = a->rowTu[r0], ntu = a->rowTu[r1] - tu0;
@@ -105,9 +194,13 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
             win.job0 = job0; win.left_count = c->d_counter + 9; win.left_list = a->d_left;
             win.order = a->d_order + job0;
         }
+        MePlanes pl;
+        pl.nrefs = a->p.numRefs; pl.ppitch = (ptrdiff_t)(a->planeBytes / (depth == 8 ? 1 : 2));
+        for (int r = 0; r < a->p.numRefs; r++) pl.blocks[r] = a->d_refs[r];
+        for (int g = 0; g < 3; g++) { pl.jobs[g] = a->d_planeJobs[g]; pl.njobs[g] = a->nPlaneJobs[g]; }
         if (launch_me(c, depth, a->d_fenc + a->orgBytes, a->stride, (const void* const*)a->d_refTable, a->stride, 0,
                       a->d_mvcost + a->mvrange, a->d_jobs + job0, nj, a->d_me_out + (size_t)job0 * 4, c->d_counter,
-                      a->chromaOn ? &ch : NULL, a->windowOn ? &win : NULL)) return -1;
+                      a->chromaOn ? &ch : NULL, a->windowOn ? &win : NULL, &pl)) return -1;
         CU_CHECK(cudaEventRecord(a->ev[4], c->stream));      // ME search kernel alone ends here
         k_pack_me<<<(nj + 255) / 256, 256, 0, c->stream>>>(a->d_me_out + (size_t)job0 * 4, nj, a->d_me_packed + job0);
         CU_LAUNCH_CHECK(c);
@@ -184,7 +277,20 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     a->d_fenc = (uint8_t*)x265cu_malloc(ctx, a->planeBytes);
     if (a->d_fenc) cudaMemset(a->d_fenc, 0, a->planeBytes);
     void* reft[16]; void* rect[4];
-    for (int r = 0; r < p->numRefs; r++) { a->d_refs[r] = (uint8_t*)x265cu_malloc(ctx, a->planeBytes); if (a->d_refs[r]) cudaMemset(a->d_refs[r], 0, a->planeBytes); reft[r] = a->d_refs[r] + a->orgBytes; }
+    // every reference is a block of 16 planes: slot 0 the reference, slots 1..15 its phase planes.  The 15 phase planes add
+    // 15 x planeBytes per reference: 561 MB at 3840x2160 8-bit with 4 references (bench.py c3), 1.40 GB at 3840x2160 10-bit
+    // with 5 (c4), 5.3 GB at 7680x4320 10-bit with 5 (c5)
+    for (int r = 0; r < p->numRefs; r++)
+    {
+        a->d_refs[r] = (uint8_t*)x265cu_malloc(ctx, 16 * a->planeBytes);
+        if (!a->d_refs[r])
+        {
+            x265cu_set_error("x265cu_analyser_create: no device memory for a reference and its 15 phase planes", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+            return NULL;
+        }
+        cudaMemset(a->d_refs[r], 0, 16 * a->planeBytes);
+        reft[r] = a->d_refs[r] + a->orgBytes;
+    }
     for (int d = 0; d < 4; d++) { a->d_recon[d] = (uint8_t*)x265cu_malloc(ctx, a->planeBytes); rect[d] = a->d_recon[d] + a->orgBytes; cudaMemset(a->d_recon[d], 0, a->planeBytes); }
     a->d_refTable = (void**)x265cu_malloc(ctx, sizeof(void*) * 16);
     a->d_reconTable = (void**)x265cu_malloc(ctx, sizeof(void*) * 4);
@@ -234,6 +340,13 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     a->h_fenc = (uint8_t*)x265cu_host_alloc((size_t)p->width * p->height * es);
     a->h_field = (int16_t*)x265cu_host_alloc(fieldBytes);
     if (!a->d_intra || !a->d_coef || !a->d_me_out || !a->h_fenc || !a->h_field) return NULL;
+    an_build_read_rects(a);
+    if (an_build_plane_jobs(a)) return NULL;
+    if (!an_planes_cover(a, 0, a->ctuRows))
+    {
+        x265cu_set_error("x265cu_analyser_create: the phase planes do not cover what the sub-pel search can read", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return NULL;
+    }
     cudaDeviceSynchronize();
     return a;
 }
@@ -246,7 +359,8 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     cudaStreamSynchronize(c->stream);
     void* bufs[] = { a->d_fenc, a->d_refTable, a->d_reconTable, a->d_field, a->d_mvcost, a->d_pus, a->d_cus, a->d_tus, a->d_cu_jobs, a->d_jobs,
                      a->d_me_out, a->d_me_packed, a->d_coef, a->d_cu_sse, a->d_cu_numsig, a->d_cu_ref, a->d_intra,
-                     a->d_groups[0], a->d_groups[1], a->d_groups[2], a->d_grpJobs[0], a->d_grpJobs[1], a->d_grpJobs[2], a->d_tmaps, a->d_left, a->d_order };
+                     a->d_groups[0], a->d_groups[1], a->d_groups[2], a->d_grpJobs[0], a->d_grpJobs[1], a->d_grpJobs[2], a->d_tmaps, a->d_left, a->d_order,
+                     a->d_planeJobs[0], a->d_planeJobs[1], a->d_planeJobs[2] };
     for (void* b : bufs) cudaFree(b);
     for (int r = 0; r < a->p.numRefs; r++) cudaFree(a->d_refs[r]);
     for (int d = 0; d < 4; d++) cudaFree(a->d_recon[d]);
@@ -449,7 +563,10 @@ int x265cu_analyser_fetch(x265cu_analyser* a, int what, void* host)
     case 3: case 4: case 5: case 6: src = a->d_recon[what - 3]; bytes = (size_t)a->stride * a->planeRows * es; break;
     case 7: src = a->d_cu_jobs; bytes = sizeof(int32_t) * a->ncu * a->p.numRefs; break;
     case 8: src = a->d_fenc; bytes = (size_t)a->stride * a->planeRows * es; break;
-    default: return -1;
+    default:
+        // 16 + 16 * ref + phase: the whole allocation of phase plane yf * 4 + xf of reference `ref` (phase 0 = the reference)
+        if (what < 16 || what >= 16 + 16 * a->p.numRefs) return -1;
+        src = a->d_refs[(what - 16) >> 4] + (size_t)((what - 16) & 15) * a->planeBytes; bytes = (size_t)a->stride * a->planeRows * es;
     }
     CU_CHECK(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));

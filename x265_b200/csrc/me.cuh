@@ -301,12 +301,13 @@ __device__ __forceinline__ int me_band_cost(const MeCtx<P>& c, int y0, int rows,
 }
 
 // subpelCompare (motion.cpp:1571-1598) for ONE candidate: luma_hpp / luma_vpp / luma_hvpp, then cmp.
-template <typename P>
-__device__ __forceinline__ int me_subpel_compare_t(const MeCtx<P>& c, int qx, int qy, bool satd)
+// PLANES: the candidate is the full-pel block of its phase plane (see me_subpel_small_t).
+template <typename P, bool PLANES = false>
+__device__ __forceinline__ int me_subpel_compare_t(const MeCtx<P>& c, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
     constexpr int DEPTH = PixTraits<P>::depth;
-    const P* r = c.ref[0] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride;
-    const int xf = qx & 3, yf = qy & 3;
+    const P* r = c.ref[0] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride + (PLANES ? ((qy & 3) * 4 + (qx & 3)) * ppitch : 0);
+    const int xf = PLANES ? 0 : qx & 3, yf = PLANES ? 0 : qy & 3;
     if (!(xf | yf))
     {
         if (!satd) return me_sad_direct(c, r);
@@ -397,8 +398,12 @@ __device__ __forceinline__ void me_load_fenc(const MeCtx<P>& c, const P* __restr
 // filtered rows to shared memory (one row segment per lane-task), then every lane produces ITS row of the
 // prediction in registers, differences it against the source row, does the horizontal half of the 4x4 Hadamards
 // in registers and the vertical half with two xor-shuffle butterflies over the 4 lanes of a tile.
-template <typename P, int NPX>
-__device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int qx, int qy, bool satd)
+// PLANES: the reference is a block of 16 phase planes `ppitch` elements apart (phase yf * 4 + xf, MePlanes): every
+// candidate is the full-pel block of its phase plane, read as aligned words, and nothing is interpolated here.
+template <typename P, int N>
+__device__ __forceinline__ void me_ld_px(const P* __restrict__ p, int (&v)[N]);
+template <typename P, int NPX, bool PLANES = false>
+__device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
     constexpr int DEPTH = PixTraits<P>::depth;
     const int lane = c.lane;
@@ -415,7 +420,7 @@ __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int q
         const int live_n = min(cpp, n - base);
         __syncwarp();
         // ---- stage 1: horizontally filtered rows of the hv candidates ----
-        for (int t0 = 0; t0 < live_n * tasksPer; t0 += 32)
+        for (int t0 = 0; t0 < (PLANES ? 0 : live_n * tasksPer); t0 += 32)
         {
             const int t = t0 + lane;
             const int tci = min((int)(t >= tasksPer) + (int)(t >= 2 * tasksPer) + (int)(t >= 3 * tasksPer), live_n - 1);
@@ -450,7 +455,8 @@ __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int q
         {
             const P* r = c.ref[0] + (mqx >> 2) + (ptrdiff_t)((mqy >> 2) + row) * c.rstride + seg * 8;
             int pr[NPX];
-            if (!(xf | yf))
+            if (PLANES) me_ld_px<P, NPX>(r + (yf * 4 + xf) * ppitch, pr);
+            else if (!(xf | yf))
             {
 #pragma unroll
                 for (int x = 0; x < NPX; x++) pr[x] = (int)__ldg(r + x);
@@ -531,14 +537,15 @@ __device__ __forceinline__ void me_load_row8(const P* __restrict__ p, int (&v)[8
 // re-use their source rows (11 rows feed 4 output rows: me_vcol4 / me_vmid4).  The PU is processed in bands of
 // BR = min(h, 1024 / w) rows (a full warp of units for w = 64 / 32 / 16 with h >= 16 / 32 / 64); hv candidates first
 // write the band's BR + 7 horizontally filtered rows to shared memory (one row segment per lane-task).
-template <typename P>
-__device__ __forceinline__ int me_subpel_big(const MeCtx<P>& c, int qx, int qy, bool satd)
+// PLANES: the candidate is the full-pel block of its phase plane (see me_subpel_small_t).
+template <typename P, bool PLANES = false>
+__device__ __forceinline__ int me_subpel_big(const MeCtx<P>& c, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
     constexpr int DEPTH = PixTraits<P>::depth;
     const int lane = c.lane;
     const int lgsegs = c.lgw - 3, segs = 1 << lgsegs;
-    const int xf = qx & 3, yf = qy & 3;
-    const P* r0 = c.ref[0] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride;
+    const int xf = PLANES ? 0 : qx & 3, yf = PLANES ? 0 : qy & 3;
+    const P* r0 = c.ref[0] + (qx >> 2) + (ptrdiff_t)(qy >> 2) * c.rstride + (PLANES ? ((qy & 3) * 4 + (qx & 3)) * ppitch : 0);
     if (!(xf | yf) && !satd) return me_sad_direct(c, r0);             // full-pel SAD: the word-wise SAD core
     int16_t* mid = c.sm->mid;
     const int BR = min(c.h, 1024 >> c.lgw);
@@ -633,24 +640,29 @@ __device__ __forceinline__ int me_subpel_big(const MeCtx<P>& c, int qx, int qy, 
     return warp_sum(acc);
 }
 
-template <typename P>
-__device__ __forceinline__ int me_subpel_multi_small(const MeCtx<P>& c, int n, int qx, int qy, bool satd)
+template <typename P, bool PLANES = false>
+__device__ __forceinline__ int me_subpel_multi_small(const MeCtx<P>& c, int n, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
-    return c.w >= 8 ? me_subpel_small_t<P, 8>(c, n, qx, qy, satd) : me_subpel_small_t<P, 4>(c, n, qx, qy, satd);
+    return c.w >= 8 ? me_subpel_small_t<P, 8, PLANES>(c, n, qx, qy, satd, ppitch) : me_subpel_small_t<P, 4, PLANES>(c, n, qx, qy, satd, ppitch);
 }
 
 // out-of-line copy for the cold multi-site users (lowres pre-check candidates, AMP sizes)
 template <typename P>
 __device__ __noinline__ int me_subpel_compare(const MeCtx<P>& c, int qx, int qy, bool satd) { return me_subpel_compare_t(c, qx, qy, satd); }
+template <typename P>
+__device__ __noinline__ int me_subpel_compare_planes(const MeCtx<P>& c, int qx, int qy, bool satd, ptrdiff_t ppitch)
+{
+    return me_subpel_compare_t<P, true>(c, qx, qy, satd, ppitch);
+}
 
 // PU classes of the sub-pel stage: 0 = small (pow2, w and h <= 16: four candidates at a time through
 // me_subpel_multi_small), 1 = everything else (one candidate at a time, banded).  CLS = -1 compiles both.
 template <typename P>
 __device__ __forceinline__ int me_subpel_class(const MeCtx<P>& c) { return (c.pow2 && c.w <= 16 && c.h <= 16) ? 0 : 1; }
 
-// distortion of up to 8 sub-pel candidates, lane i (< n) owns candidate i; result in lane i
-template <typename P, int CLS>
-__device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx, int qy, bool satd)
+// distortion of up to 8 sub-pel candidates, lane i (< n) owns candidate i; result in lane i.  PLANES: on phase planes
+template <typename P, int CLS, bool PLANES = false>
+__device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
     int out = 0;
     if (CLS == 0 || (CLS < 0 && me_subpel_class(c) == 0))
@@ -659,7 +671,7 @@ __device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx,
         {
             const int src = min(base + (c.lane & 3), n - 1);
             const int bqx = __shfl_sync(0xffffffffu, qx, src), bqy = __shfl_sync(0xffffffffu, qy, src);
-            int v = me_subpel_multi_small(c, min(4, n - base), bqx, bqy, satd);
+            int v = me_subpel_multi_small<P, PLANES>(c, min(4, n - base), bqx, bqy, satd, ppitch);
             v = __shfl_sync(0xffffffffu, v, (c.lane - base) & 3);
             if (c.lane >= base && c.lane < base + 4) out = v;
         }
@@ -669,7 +681,8 @@ __device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx,
         for (int k = 0; k < n; k++)
         {
             const int kqx = __shfl_sync(0xffffffffu, qx, k), kqy = __shfl_sync(0xffffffffu, qy, k);
-            int v = c.pow2 ? me_subpel_big(c, kqx, kqy, satd) : me_subpel_compare(c, kqx, kqy, satd);      // AMP sizes: generic, out of line
+            int v = c.pow2 ? me_subpel_big<P, PLANES>(c, kqx, kqy, satd, ppitch)
+                           : PLANES ? me_subpel_compare_planes(c, kqx, kqy, satd, ppitch) : me_subpel_compare(c, kqx, kqy, satd);   // AMP sizes: generic, out of line
             if (c.lane == k) out = v;
         }
     }
@@ -1527,8 +1540,10 @@ __device__ __forceinline__ void me_phase2(MeCtx<P>& c, const x265cu_me_job& j, M
 }
 
 // phase 3 (motion.cpp:1440-1569): pick pre-check vs search winner, sub-pel refinement
-template <typename P, int CLS, bool CHROMA = false>
-__device__ __forceinline__ void me_phase3(MeCtx<P>& c, const x265cu_me_job& j, const MeState& st, int32_t* __restrict__ out, const MeChromaCtx<P>* cc = nullptr)
+// PLANES: the luma distortion of every candidate comes from the reference's phase planes (MePlanes), `ppitch` apart
+template <typename P, int CLS, bool CHROMA = false, bool PLANES = false>
+__device__ __forceinline__ void me_phase3(MeCtx<P>& c, const x265cu_me_job& j, const MeState& st, int32_t* __restrict__ out, const MeChromaCtx<P>* cc = nullptr,
+                                          ptrdiff_t ppitch = 0)
 {
     const int qminy = c.miny * 4, qmaxy = c.maxy * 4;
     int bcost = st.bcost;
@@ -1583,7 +1598,7 @@ __device__ __forceinline__ void me_phase3(MeCtx<P>& c, const x265cu_me_job& j, c
             int qx = bx + c_square1[i1][0] * step, qy = by + c_square1[i1][1] * step, dir = i1, dummy = 0;
             const bool valid = c.lane < dirs && (centre || !((qy < qminy) | (qy > qmaxy)));
             const int n = me_compact(valid, dirs, qx, qy, dir, dummy);
-            int cost = me_subpel_batch<P, CLS>(c, n, qx, qy, satd);
+            int cost = me_subpel_batch<P, CLS, PLANES>(c, n, qx, qy, satd, ppitch);
             if (CHROMA && cc->on)
             {
                 const int ccost = me_chroma_batch<P, CLS>(c, *cc, n, qx, qy, n >= 32 ? 0xffffffffu : ((1u << n) - 1u));
@@ -1642,12 +1657,14 @@ constexpr int ME_P2_BLOCKS = 4, ME_MIN_BLOCKS = 3, ME_BIG_BLOCKS = 2;
 // CHROMA: the pre-check and sub-pel launches with the chroma-SATD term (x265cu_me_batch_chroma), separate instantiations so
 // that the luma-only kernels carry no chroma code.  They run full-resolution planes only (the lowres planes have no
 // chroma), and the integer search (phase 2) is luma only in the reference too.
-template <typename P, int PHASE, int CLS, bool CHROMA>
+// PLANES (sub-pel phase only): the references are blocks of phase planes `ppitch` elements apart (MePlanes); these
+// instantiations have no interpolation code and use no MeShared scratch.
+template <typename P, int PHASE, int CLS, bool CHROMA, bool PLANES = false>
 __global__ void __launch_bounds__(256, PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS)) k_me(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, int lowres,
                                                            MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs, int n,
                                                            int32_t* __restrict__ out, MeState* __restrict__ state, int* __restrict__ counter,
                                                            const int32_t* __restrict__ list, const int* __restrict__ list_n,
-                                                           const int32_t* __restrict__ order, int order0)
+                                                           const int32_t* __restrict__ order, int order0, ptrdiff_t ppitch)
 {
     extern __shared__ unsigned char me_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1674,26 +1691,30 @@ __global__ void __launch_bounds__(256, PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? M
         if (PHASE != 1) st = state[jid];
         if (PHASE == 1) { me_phase1<P, CLS, CHROMA>(c, j, st, &cc); if (lane == 0) state[jid] = st; }
         if (PHASE == 2) { me_phase2<P>(c, j, st); if (lane == 0) state[jid] = st; }
-        if (PHASE == 3) me_phase3<P, CLS, CHROMA>(c, j, st, out + (size_t)jid * 4, &cc);
+        if (PHASE == 3) me_phase3<P, CLS, CHROMA, PLANES>(c, j, st, out + (size_t)jid * 4, &cc, ppitch);
         __syncwarp();
     }
 }
 
-// One launch of k_me; `ch` != NULL selects the chroma instantiation (pre-check and sub-pel phases only)
+// One launch of k_me; `ch` != NULL selects the chroma instantiation (pre-check and sub-pel phases only), `ppitch` != 0
+// the phase-plane one (sub-pel phase only)
 template <typename P, int PHASE, int CLS>
 static int launch_me_phase(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres, const MeChromaArgs* ch,
                            const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, MeState* state, int* counter,
-                           const int32_t* list, const int* list_n, const int32_t* order, int order0)
+                           const int32_t* list, const int* list_n, const int32_t* order, int order0, ptrdiff_t ppitch = 0)
 {
     const int threads = 256, warps = threads / 32;
-    const size_t smem = PHASE == 2 ? 0 : sizeof(MeShared) * warps;      // the integer search never touches the interpolation scratch
+    const bool planes = PHASE == 3 && ppitch != 0;
+    // the integer search and the phase-plane sub-pel kernels never touch the interpolation scratch
+    const size_t smem = PHASE == 2 || planes ? 0 : sizeof(MeShared) * warps;
     int blocks = ctx->sm_count * (PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? ME_BIG_BLOCKS : ME_MIN_BLOCKS));
     int need = (n + warps - 1) / warps;
     if (blocks > need) blocks = need;
     const MeChromaArgs none = {};
-    const auto kernel = ch ? k_me<P, PHASE, CLS, PHASE != 2> : k_me<P, PHASE, CLS, false>;
+    const auto kernel = planes ? (ch ? k_me<P, PHASE, CLS, PHASE != 2, PHASE == 3> : k_me<P, PHASE, CLS, false, PHASE == 3>)
+                               : (ch ? k_me<P, PHASE, CLS, PHASE != 2> : k_me<P, PHASE, CLS, false>);
     kernel<<<blocks, threads, smem, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, lowres, ch ? *ch : none, mvcost, jobs, n, out,
-                                                   state, counter, list, list_n, order, order0);
+                                                   state, counter, list, list_n, order, order0, ppitch);
     CU_LAUNCH_CHECK(ctx);
     return 0;
 }
@@ -1716,10 +1737,38 @@ template <typename P>
 static int launch_me_precheck_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs* ch,
                                      const uint16_t* mvcost, const x265cu_me_job* jobs, MeState* st, const MeWinLaunch& w, int* left_count, int32_t* left_list);
 
+// Quarter-pel phase planes of the references (the frame analyser, analyser.cuh): every reference is one block of 16 planes
+// `ppitch` elements apart with the reference's stride and origin; slot yf * 4 + xf holds the luma plane interpolated at
+// phase (xf, yf) exactly as luma_hpp / luma_vpp / luma_hvpp compute it (ipfilter.cpp:79-369), slot 0 is the reference
+// itself.  launch_me builds slots 1..15 right before the sub-pel launches, from tile jobs (k_interp_rows) that are the
+// same for every reference; the sub-pel launches then read every candidate as the full-pel block of its phase plane.
+struct MePlanes
+{
+    uint8_t* blocks[16]; int nrefs;                         // block base (= slot 0 allocation) of every reference
+    ptrdiff_t ppitch;                                       // elements from one phase plane to the next
+    const x265cu_interp_job* jobs[3]; int njobs[3];         // device tile jobs of the hpp / vpp / hvpp phases
+};
+
+template <typename P>
+static int me_build_planes(x265cu_ctx* ctx, const MePlanes& pl)
+{
+    static const int ops[3] = { X265CU_HPP, X265CU_VPP, X265CU_HVPP };
+    for (int r = 0; r < pl.nrefs; r++)
+        for (int g = 0; g < 3; g++)
+        {
+            if (pl.njobs[g] <= 0) continue;
+            int fb = (pl.njobs[g] + 7) / 8;
+            if (fb > ctx->sm_count * 8) fb = ctx->sm_count * 8;
+            launch_interp_rows<P>(ctx, fb, ops[g], pl.blocks[r], pl.blocks[r], pl.jobs[g], pl.njobs[g]);
+            CU_LAUNCH_CHECK(ctx);
+        }
+    return 0;
+}
+
 template <typename P>
 static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres,
                        const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, MeState* st, int* counter_dev,
-                       const MeChromaArgs* ch, const MeWinLaunch* win)
+                       const MeChromaArgs* ch, const MeWinLaunch* win, const MePlanes* planes)
 {
     int rc = 0;
     // with job groups (the frame analyser), the pre-checks of the 16x16 cells come out of shared per-cell tables
@@ -1740,14 +1789,17 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
     if (grp) rc |= launch_me_window<P>(ctx, fenc, fstride, mvcost, jobs, st, *win);
     rc |= launch_me_phase<P, 2, -1>(ctx, fenc, fstride, refs, rstride, lowres, NULL, mvcost, jobs, n, out, st, counter_dev + 2, left, left_n, NULL, 0);
     CU_CHECK(cudaEventRecord(ctx->me_ev[2], ctx->stream));
-    rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0);
-    rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0);
+    // the phase planes are built inside the sub-pel phase, so its time includes them
+    const ptrdiff_t pp = planes && !lowres ? planes->ppitch : 0;
+    if (pp) rc |= me_build_planes<P>(ctx, *planes);
+    rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0, pp);
+    rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0, pp);
     return rc;
 }
 
 static int launch_me(x265cu_ctx* ctx, int depth, const void* fenc, int fstride, const void* const* refs, int rstride, int lowres,
                      const uint16_t* mvcost, const x265cu_me_job* jobs, int n, int32_t* out, int* counter_dev, const MeChromaArgs* chroma = NULL,
-                     const MeWinLaunch* win = NULL)
+                     const MeWinLaunch* win = NULL, const MePlanes* planes = NULL)
 {
     if (n <= 0) return 0;
     CU_CHECK(cudaMemsetAsync(counter_dev, 0, 8 * sizeof(int), ctx->stream));
@@ -1762,8 +1814,8 @@ static int launch_me(x265cu_ctx* ctx, int depth, const void* fenc, int fstride, 
     MeState* st = (MeState*)ctx->d_me_state;
     CU_CHECK(cudaEventRecord(ctx->me_ev[0], ctx->stream));
     if (chroma && lowres) chroma = NULL;                    // the lowres planes have no chroma (lowres.h)
-    const int rc = depth == 8 ? launch_me_t<uint8_t>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev, chroma, win)
-                              : launch_me_t<uint16_t>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev, chroma, win);
+    const int rc = depth == 8 ? launch_me_t<uint8_t>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev, chroma, win, planes)
+                              : launch_me_t<uint16_t>(ctx, fenc, fstride, refs, rstride, lowres, mvcost, jobs, n, out, st, counter_dev, chroma, win, planes);
     CU_CHECK(cudaEventRecord(ctx->me_ev[3], ctx->stream));
     return rc;
 }

@@ -412,8 +412,16 @@ class Analyser:
         self.lib.check(self.lib.L.x265cu_analyser_ref_updated(self.h, idx))
 
     def fetch(self, what):
+        """A device-resident array by name, or ("plane", ref, phase): the whole allocation (stride x (height + 160)) of
+        reference ref's phase plane yf * 4 + xf (phase 0 = the reference plane itself)."""
         es = np.dtype(self.dtype).itemsize
         rows = self.height + 160
+        if isinstance(what, tuple):
+            _, ref, phase = what
+            assert 0 <= ref < self.numRefs and 0 <= phase < 16, what
+            out = np.zeros((rows, self.stride), self.dtype)
+            self.lib.check(self.lib.L.x265cu_analyser_fetch(self.h, 16 + 16 * ref + phase, out.ctypes.data))
+            return out
         spec = {"jobs": (0, ME_JOB, self.njobs), "me_out": (1, np.int32, self.njobs * 4), "coef": (2, np.int16, self.ncoef),
                 "recon0": (3, self.dtype, self.stride * rows), "recon1": (4, self.dtype, self.stride * rows),
                 "recon2": (5, self.dtype, self.stride * rows), "recon3": (6, self.dtype, self.stride * rows),
