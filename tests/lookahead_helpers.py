@@ -65,7 +65,7 @@ class OracleLookahead:
             planes, ls, lorg, w8, h8 = make_lowres(O, img, depth)
             ncu = w8 * h8
             f = dict(planes=planes, intraCost=np.zeros(ncu, np.int32), intraMode=np.zeros(ncu, np.uint8),
-                     lowresCosts={}, rowSatds={}, costEst={}, mvs={}, mvcosts={}, intraMbs={})
+                     lowresCosts={}, rowSatds={}, costEst={}, mvs={}, mvcosts={}, intraMbs={}, estIntraMbs={})
             lc = np.zeros(ncu, np.uint16); rs = np.zeros(h8, np.int32); ce = np.zeros(2, np.int64)
             O.orc_lowres_intra(ptr(planes[0], lorg), IP(ls), w8, h8, int(self.lam), ptr(invq[fi]) if invq is not None else None, ptr(f["intraCost"]), ptr(f["intraMode"]), ptr(lc), ptr(rs), ptr(ce))
             f["lowresCosts"][(0, 0)] = lc; f["rowSatds"][(0, 0)] = rs; f["costEst"][(0, 0)] = (int(ce[0]), int(ce[1]))
@@ -109,4 +109,5 @@ class OracleLookahead:
             score = score * 100 // 130          # slicetype.cpp:3205-3206, bFrameBias = 0
         f["lowresCosts"][(d0, d1)] = lc; f["rowSatds"][(d0, d1)] = rs
         f["costEst"][(d0, d1)] = (score, int(j.out[1])); f["intraMbs"][d0] = f["intraMbs"].get(d0, 0) + int(j.out[2])
+        f["estIntraMbs"][(d0, d1)] = int(j.out[2])      # this estimate's own count (intraMbs[d0] sums the estimates at d0)
         return score

@@ -55,9 +55,11 @@ def test_lookahead_gpu(cu, depth, size, noise):
         assert np.array_equal(gpu.fr[b]["mvcosts"][(0, d0)].download(np.int32), orc.fr[b]["mvcosts"][(0, d0)])
         if p1 > b:
             assert np.array_equal(gpu.fr[b]["mvs"][(1, d1)].download(np.int32).reshape(-1, 2), orc.fr[b]["mvs"][(1, d1)])
+            assert np.array_equal(gpu.fr[b]["mvcosts"][(1, d1)].download(np.int32), orc.fr[b]["mvcosts"][(1, d1)])
         assert np.array_equal(r["lowresCosts"], orc.fr[b]["lowresCosts"][(d0, d1)]), (p0, p1, b)
         assert np.array_equal(r["rowSatds"], orc.fr[b]["rowSatds"][(d0, d1)])
         assert a == c and r["costEstAq"] == orc.fr[b]["costEst"][(d0, d1)][1], ((p0, p1, b), a, c)
+        assert r["intraMbs"] == orc.fr[b]["estIntraMbs"][(d0, d1)], ((p0, p1, b), r["intraMbs"])
 
 
 @pytest.mark.parametrize("world", [2, 4])

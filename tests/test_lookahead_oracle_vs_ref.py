@@ -13,6 +13,10 @@ from lookahead_helpers import OracleLookahead
 from ref_results import RefResults
 
 TRIPLES = [(0, 1, 1), (0, 2, 1), (0, 2, 2), (0, 3, 1), (0, 3, 2), (0, 3, 3), (1, 3, 2), (2, 3, 3)]
+# whole-frame geometries of tests/test_gpu_lookahead_shapes.py (lowres CU grids 120x68, 240x135, 130x65, 128x64, 68x120,
+# 240x4, 4x135): 1080p and 2160p as presets medium to slower run them, the diagonal-length edges of the device wavefront,
+# a portrait frame and the narrowest legal strips (64 px, the smallest picture at CTU 64, param.cpp:1597)
+SHAPE_SIZES = [(1920, 1080), (3840, 2160), (2080, 1040), (2048, 1024), (1080, 1920), (3840, 64), (64, 2160)]
 
 
 class RefLookahead:
@@ -56,7 +60,7 @@ class RefLookahead:
 
 
 @pytest.mark.parametrize("depth", [8, 10])
-@pytest.mark.parametrize("size,noise", [((416, 240), False), ((200, 136), True)])
+@pytest.mark.parametrize("size,noise", [((416, 240), False), ((200, 136), True)] + [(s, False) for s in SHAPE_SIZES])
 def test_lookahead(depth, size, noise, request):
     G = RefResults(request, depth)
     O = load_oracle(depth)
@@ -96,9 +100,19 @@ def test_lookahead_cooperative_slices(depth, lslices, request):
     """estimateFrameCost as presets medium / slow run it (param.cpp:173 lookaheadSlices 8, :492 slow 4): the cooperative-slice
     path (slicetype.cpp:3075-3112, 3143-3173) of the REAL Lookahead (a pool without running workers: the caller processes
     every slice) against the oracle's slice loop -- frame costs, per-CU costs, row sums and motion fields."""
+    _cooperative_slices(request, depth, lslices, 1280, 720)     # slices need a source height >= 720 (slicetype.cpp:1022-1026)
+
+
+@pytest.mark.parametrize("depth,size,lslices", [(8, (1920, 1080), 8), (8, (3840, 2160), 4)], ids=["medium", "slow_2160"])
+def test_lookahead_cooperative_slices_geometries(depth, size, lslices, request):
+    """The cooperative-slice path at 1080p with preset medium's 8 slices (6 of 10 CU rows, the last of 18) and at 2160p with
+    preset slow's 4 (33 / 33 / 33 / 36 rows): the geometries tests/test_gpu_lookahead_shapes.py runs on the device."""
+    _cooperative_slices(request, depth, lslices, *size)
+
+
+def _cooperative_slices(request, depth, lslices, W, H):
     G = RefResults(request, depth)
     O = load_oracle(depth)
-    W, H = 1280, 720                                  # slices need a source height >= 720 (slicetype.cpp:1022-1026)
     frames = [gen_luma(W, H, i, bits=depth) for i in range(3)]
     ref = RefLookahead(G.R, frames, lslices=lslices) if G.R else None
     slices = tuple(int(x) for x in G.value("slices", lambda: ref.slices))
