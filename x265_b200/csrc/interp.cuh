@@ -107,6 +107,22 @@ __device__ __forceinline__ void me_hrow(const P* __restrict__ s, int xf, int (&s
     }
 }
 
+// Stage 1 of hv (hps with rowExt, ipfilter.cpp:120-162) for the NPX outputs starting at pixel s: the horizontal sums
+// rounded to the 14-bit intermediate, stored packed at d (one 16-byte store for 8 outputs, 8 bytes for 4).
+template <typename P, int NPX>
+__device__ __forceinline__ void me_hv_row(const P* __restrict__ s, int xf, int16_t* __restrict__ d)
+{
+    constexpr int DEPTH = PixTraits<P>::depth;
+    int sum[NPX];
+    me_hrow<P, NPX>(s, xf, sum);
+    uint32_t pk[NPX / 2];
+#pragma unroll
+    for (int i = 0; i < NPX / 2; i++)
+        pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
+    if (NPX == 8) *(uint4*)d = make_uint4(pk[0], pk[1], pk[NPX / 2 - 2], pk[NPX / 2 - 1]);
+    else          *(uint2*)d = make_uint2(pk[0], pk[NPX / 2 - 1]);
+}
+
 // NPX vertical 8-tap sums straight from pixel rows; s = (row y-3, first pixel of the segment).  8-bit: each
 // 4x4 block of bytes is transposed in registers (8 PRMT) so that a pixel's four vertical taps are one DP4A.
 template <typename P, int NPX>
@@ -450,13 +466,7 @@ __global__ void __launch_bounds__(256) k_interp_rows(int op, const P* __restrict
                 for (int t = lane; t < (rows + 7) * segs; t += 32)
                 {
                     const int mrow = t / segs, seg = t - mrow * segs;
-                    int sum[8];
-                    me_hrow<P, 8>(s0 + (ptrdiff_t)(y0 - 3 + mrow) * jb.s_stride + seg * 8, jb.idxX, sum);
-                    uint32_t pk[4];
-#pragma unroll
-                    for (int i = 0; i < 4; i++)
-                        pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
-                    *(uint4*)(mid + mrow * w + seg * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                    me_hv_row<P, 8>(s0 + (ptrdiff_t)(y0 - 3 + mrow) * jb.s_stride + seg * 8, jb.idxX, mid + mrow * w + seg * 8);
                 }
                 __syncwarp();
                 for (int u = lane; u < rows * segs; u += 32)

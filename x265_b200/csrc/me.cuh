@@ -37,6 +37,8 @@ struct MeCtx
     int nw, lgnw, lgwpr;                   // words per PU, log2, log2(words per row)
     int lgsegw;                            // log2 words per lane segment (16 B when the fenc rows allow vector loads)
     MeShared* sm;
+    static constexpr bool startsOutside = true;     // a star may start outside the range (MV 0 won the pre-checks)
+    static constexpr bool hasStarTable = false;
 };
 
 // mvcost of the qpel vector (qx, qy) against the predictor (mvpx, mvpy): `mvc` is the centred table
@@ -390,6 +392,79 @@ __device__ __forceinline__ void me_load_fenc(const MeCtx<P>& c, const P* __restr
     }
 }
 
+template <typename P, int N>
+__device__ __forceinline__ void me_ld_px(const P* __restrict__ p, int (&v)[N]);
+
+// NPX predicted values of one row segment of a candidate at phase (xf, yf): r = the segment's full-pel position in the
+// reference, m = the same segment in the hv candidate's horizontally filtered rows (me_hv_row, `mpitch` elements per row).
+// The pixel prediction of luma_hpp / luma_vpp / luma_hvpp, or with SHORT the 14-bit intermediate of predInterLumaShort
+// (p2s / hps / vps / hps + vss).
+template <typename P, int NPX, bool SHORT>
+__device__ __forceinline__ void me_pred_seg(const P* __restrict__ r, int rstride, int xf, int yf, const int16_t* __restrict__ m, int mpitch,
+                                            int (&pr)[NPX])
+{
+    constexpr int DEPTH = PixTraits<P>::depth;
+    if (!(xf | yf))
+    {
+#pragma unroll
+        for (int x = 0; x < NPX; x++) { const int p = (int)__ldg(r + x); pr[x] = SHORT ? (p << (14 - DEPTH)) - 8192 : p; }
+    }
+    else if (!yf)
+    {
+        me_hrow<P, NPX>(r, xf, pr);
+#pragma unroll
+        for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 1 : 0);
+    }
+    else if (!xf)
+    {
+        me_vcol<P, NPX>(r - 3 * (ptrdiff_t)rstride, rstride, yf, pr);
+#pragma unroll
+        for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 1 : 0);
+    }
+    else
+    {
+        me_vmid<NPX>(m, mpitch, yf, pr);
+#pragma unroll
+        for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 3 : 2);
+    }
+}
+
+// Distortion of a candidate whose row-segment differences d are spread over `lpc` lanes (lane = row + h * segment, so the
+// 4 lanes of a 4-row tile are consecutive): SAD, or SATD with the horizontal 4-point Hadamards in registers, the vertical ones
+// over the 4 lanes of a tile, each 8x4 (4x4) tile halved on its own.  Every lane of the candidate gets the sum.
+template <int NPX>
+__device__ __forceinline__ int me_seg_cost(int (&d)[NPX], bool satd, int lane, int lpc)
+{
+    int part = 0;
+    if (!satd)
+    {
+#pragma unroll
+        for (int x = 0; x < NPX; x++) part += abs(d[x]);
+        for (int o = 1; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+        return part;
+    }
+#pragma unroll
+    for (int x = 0; x < NPX; x += 4) had4(d[x], d[x + 1], d[x + 2], d[x + 3]);
+#pragma unroll
+    for (int st = 1; st <= 2; st <<= 1)
+    {
+        const bool up = (lane & st) != 0;
+#pragma unroll
+        for (int x = 0; x < NPX; x++)
+        {
+            const int o = __shfl_xor_sync(0xffffffffu, d[x], st);
+            d[x] = up ? o - d[x] : o + d[x];
+        }
+    }
+#pragma unroll
+    for (int x = 0; x < NPX; x++) part += abs(d[x]);
+    part += __shfl_xor_sync(0xffffffffu, part, 1);
+    part += __shfl_xor_sync(0xffffffffu, part, 2);
+    part = (lane & 3) ? 0 : (part >> 1);                        // one 8x4 (4x4) tile per 4 lanes, halved per tile
+    for (int o = 4; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    return part;
+}
+
 // Up to 4 sub-pel candidates of a SMALL PU, lane i (< n <= 4) owns candidate i (qx, qy) and gets its distortion.
 // Per candidate the arithmetic is exactly subpelCompare's (motion.cpp:1571-1598: luma_hpp / luma_vpp / luma_hvpp
 // = hps(rowExt) + vsp, ipfilter.cpp:79-369) followed by sad or satd (8x4 tiles, 4x4 for w = 4; pixel.cpp:263-297).
@@ -400,8 +475,6 @@ __device__ __forceinline__ void me_load_fenc(const MeCtx<P>& c, const P* __restr
 // in registers and the vertical half with two xor-shuffle butterflies over the 4 lanes of a tile.
 // PLANES: the reference is a block of 16 phase planes `ppitch` elements apart (phase yf * 4 + xf, MePlanes): every
 // candidate is the full-pel block of its phase plane, read as aligned words, and nothing is interpolated here.
-template <typename P, int N>
-__device__ __forceinline__ void me_ld_px(const P* __restrict__ p, int (&v)[N]);
 template <typename P, int NPX, bool PLANES = false>
 __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
@@ -430,16 +503,8 @@ __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int q
             if (t < live_n * tasksPer && txf && tyf)
             {
                 const int mrow = tt >> lgsegs, seg = tt & ((1 << lgsegs) - 1);
-                const P* s = c.ref[0] + (tqx >> 2) + (ptrdiff_t)((tqy >> 2) - 3 + mrow) * c.rstride + seg * 8;
-                int sum[NPX];
-                me_hrow<P, NPX>(s, txf, sum);
-                uint32_t pk[NPX / 2];
-#pragma unroll
-                for (int i = 0; i < NPX / 2; i++)
-                    pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
-                int16_t* d = mid + tci * midPer + mrow * c.w + seg * 8;
-                if (NPX == 8) *(uint4*)d = make_uint4(pk[0], pk[1], pk[NPX / 2 - 2], pk[NPX / 2 - 1]);
-                else          *(uint2*)d = make_uint2(pk[0], pk[NPX / 2 - 1]);
+                me_hv_row<P, NPX>(c.ref[0] + (tqx >> 2) + (ptrdiff_t)((tqy >> 2) - 3 + mrow) * c.rstride + seg * 8, txf,
+                                  mid + tci * midPer + mrow * c.w + seg * 8);
             }
         }
         __syncwarp();
@@ -454,6 +519,8 @@ __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int q
         if (live)
         {
             const P* r = c.ref[0] + (mqx >> 2) + (ptrdiff_t)((mqy >> 2) + row) * c.rstride + seg * 8;
+            // written out rather than through me_pred_seg: with the helper the hv scratch address is formed ahead of the
+            // branch and the chroma sub-pel kernel (80 registers) spills
             int pr[NPX];
             if (PLANES) me_ld_px<P, NPX>(r + (yf * 4 + xf) * ppitch, pr);
             else if (!(xf | yf))
@@ -490,35 +557,7 @@ __device__ __forceinline__ int me_subpel_small_t(const MeCtx<P>& c, int n, int q
             for (int x = 0; x < NPX; x++) d[x] = 0;
         }
         // ---- stage 3: distortion ----
-        int part = 0;
-        if (!satd)
-        {
-#pragma unroll
-            for (int x = 0; x < NPX; x++) part += abs(d[x]);
-            for (int o = 1; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        }
-        else
-        {
-#pragma unroll
-            for (int x = 0; x < NPX; x += 4) had4(d[x], d[x + 1], d[x + 2], d[x + 3]);
-#pragma unroll
-            for (int st = 1; st <= 2; st <<= 1)
-            {
-                const bool up = (lane & st) != 0;
-#pragma unroll
-                for (int x = 0; x < NPX; x++)
-                {
-                    const int o = __shfl_xor_sync(0xffffffffu, d[x], st);
-                    d[x] = up ? o - d[x] : o + d[x];
-                }
-            }
-#pragma unroll
-            for (int x = 0; x < NPX; x++) part += abs(d[x]);
-            part += __shfl_xor_sync(0xffffffffu, part, 1);
-            part += __shfl_xor_sync(0xffffffffu, part, 2);
-            part = (lane & 3) ? 0 : (part >> 1);                    // one 8x4 (4x4) tile per 4 lanes, halved per tile
-            for (int o = 4; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        }
+        const int part = me_seg_cost<NPX>(d, satd, lane, lpc);
         const int v = __shfl_sync(0xffffffffu, part, ((lane - base) << lglpc) & 31);
         if (lane >= base && lane < base + live_n) out = v;
     }
@@ -560,13 +599,7 @@ __device__ __forceinline__ int me_subpel_big(const MeCtx<P>& c, int qx, int qy, 
             for (int t = lane; t < tasks; t += 32)
             {
                 const int mrow = t >> lgsegs, seg = t & (segs - 1);
-                int sum[8];
-                me_hrow<P, 8>(r0 + (ptrdiff_t)(y0 - 3 + mrow) * c.rstride + seg * 8, xf, sum);
-                uint32_t pk[4];
-#pragma unroll
-                for (int i = 0; i < 4; i++)
-                    pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
-                *(uint4*)(mid + mrow * c.w + seg * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                me_hv_row<P, 8>(r0 + (ptrdiff_t)(y0 - 3 + mrow) * c.rstride + seg * 8, xf, mid + mrow * c.w + seg * 8);
             }
             __syncwarp();
         }
@@ -660,22 +693,30 @@ __device__ __noinline__ int me_subpel_compare_planes(const MeCtx<P>& c, int qx, 
 template <typename P>
 __device__ __forceinline__ int me_subpel_class(const MeCtx<P>& c) { return (c.pow2 && c.w <= 16 && c.h <= 16) ? 0 : 1; }
 
+// Up to 8 candidates four at a time, lane i (< n) owns candidate i and gets its result: per pass, lanes 0-3 hold the pass's
+// candidates and `eval(m, qx, qy)` returns the distortion of candidate i (< m <= 4) in lane i.
+template <typename F>
+__device__ __forceinline__ int me_batch4(int n, int qx, int qy, int lane, F eval)
+{
+    int out = 0;
+    for (int base = 0; base < n; base += 4)
+    {
+        const int src = min(base + (lane & 3), n - 1);
+        const int bqx = __shfl_sync(0xffffffffu, qx, src), bqy = __shfl_sync(0xffffffffu, qy, src);
+        int v = eval(min(4, n - base), bqx, bqy);
+        v = __shfl_sync(0xffffffffu, v, (lane - base) & 3);
+        if (lane >= base && lane < base + 4) out = v;
+    }
+    return out;
+}
+
 // distortion of up to 8 sub-pel candidates, lane i (< n) owns candidate i; result in lane i.  PLANES: on phase planes
 template <typename P, int CLS, bool PLANES = false>
 __device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx, int qy, bool satd, ptrdiff_t ppitch = 0)
 {
     int out = 0;
     if (CLS == 0 || (CLS < 0 && me_subpel_class(c) == 0))
-    {
-        for (int base = 0; base < n; base += 4)
-        {
-            const int src = min(base + (c.lane & 3), n - 1);
-            const int bqx = __shfl_sync(0xffffffffu, qx, src), bqy = __shfl_sync(0xffffffffu, qy, src);
-            int v = me_subpel_multi_small<P, PLANES>(c, min(4, n - base), bqx, bqy, satd, ppitch);
-            v = __shfl_sync(0xffffffffu, v, (c.lane - base) & 3);
-            if (c.lane >= base && c.lane < base + 4) out = v;
-        }
-    }
+        out = me_batch4(n, qx, qy, c.lane, [&](int m, int bqx, int bqy) { return me_subpel_multi_small<P, PLANES>(c, m, bqx, bqy, satd, ppitch); });
     else
     {
         for (int k = 0; k < n; k++)
@@ -687,32 +728,6 @@ __device__ __forceinline__ int me_subpel_batch(const MeCtx<P>& c, int n, int qx,
         }
     }
     return out;
-}
-
-// SATD partial of one row segment: horizontal 4-point Hadamards in registers, vertical ones over the 4 lanes of a
-// tile; returns the halved tile sum in the tile's first lane (0 elsewhere)
-template <int NPX>
-__device__ __forceinline__ int me_seg_satd(int (&d)[NPX], int lane)
-{
-#pragma unroll
-    for (int x = 0; x < NPX; x += 4) had4(d[x], d[x + 1], d[x + 2], d[x + 3]);
-#pragma unroll
-    for (int st = 1; st <= 2; st <<= 1)
-    {
-        const bool up = (lane & st) != 0;
-#pragma unroll
-        for (int x = 0; x < NPX; x++)
-        {
-            const int o = __shfl_xor_sync(0xffffffffu, d[x], st);
-            d[x] = up ? o - d[x] : o + d[x];
-        }
-    }
-    int part = 0;
-#pragma unroll
-    for (int x = 0; x < NPX; x++) part += abs(d[x]);
-    part += __shfl_xor_sync(0xffffffffu, part, 1);
-    part += __shfl_xor_sync(0xffffffffu, part, 2);
-    return (lane & 3) ? 0 : (part >> 1);                 // one 8x4 (4x4) tile per 4 lanes, halved per tile
 }
 
 // 8 pixels of a reference row at any byte phase
@@ -767,16 +782,7 @@ __device__ __forceinline__ int me_lowres_multi(const MeCtx<P>& c, int n, int qx,
 #pragma unroll
         for (int x = 0; x < 8; x++) d[x] = slot < n ? fv[x] - a[x] : 0;
     }
-    int part = 0;
-    if (!satd)
-    {
-#pragma unroll
-        for (int x = 0; x < 8; x++) part += abs(d[x]);
-        part += __shfl_xor_sync(0xffffffffu, part, 1);
-        part += __shfl_xor_sync(0xffffffffu, part, 2);
-    }
-    else part = me_seg_satd<8>(d, lane);
-    part += __shfl_xor_sync(0xffffffffu, part, 4);
+    const int part = me_seg_cost<8>(d, satd, lane, 8);
     return __shfl_sync(0xffffffffu, part, (lane << 3) & 31);
 }
 
@@ -784,16 +790,7 @@ __device__ __forceinline__ int me_lowres_multi(const MeCtx<P>& c, int n, int qx,
 template <typename P>
 __device__ __forceinline__ int me_lowres_batch(const MeCtx<P>& c, int n, int qx, int qy, bool satd)
 {
-    int out = 0;
-    for (int base = 0; base < n; base += 4)
-    {
-        const int src = min(base + (c.lane & 3), n - 1);
-        const int bqx = __shfl_sync(0xffffffffu, qx, src), bqy = __shfl_sync(0xffffffffu, qy, src);
-        int v = me_lowres_multi(c, min(4, n - base), bqx, bqy, satd);
-        v = __shfl_sync(0xffffffffu, v, (c.lane - base) & 3);
-        if (c.lane >= base && c.lane < base + 4) out = v;
-    }
-    return out;
+    return me_batch4(n, qx, qy, c.lane, [&](int m, int bqx, int bqy) { return me_lowres_multi(c, m, bqx, bqy, satd); });
 }
 
 struct MeStar { int bx, by, bcost, point, dist; };
@@ -863,21 +860,9 @@ __device__ __forceinline__ void me_star_point(int mylvl, int k, int ox, int oy, 
     }
 }
 
-// Hooks of the shared-memory-window search (me_window.cuh): the first star round of a 16x16 cell's PUs that start at the
-// same point reads its candidates' SADs from a table computed once per cell.  Global-memory contexts never have one.
-template <typename P> __device__ __forceinline__ bool me_star_cached(const MeCtx<P>&) { return false; }
-template <typename P> __device__ __forceinline__ int me_star_lookup(const MeCtx<P>&, int, int, int, int) { return 0; }
-template <typename P> struct MeWinCell;
-template <typename P> __device__ __forceinline__ bool me_star_cached(const MeWin<P>&);
-template <typename P> __device__ __forceinline__ int me_star_lookup(const MeWin<P>&, int, int, int, int);
-template <typename P> __device__ __forceinline__ bool me_star_cached(const MeWinCell<P>& c);
-template <typename P> __device__ __forceinline__ int me_star_lookup(const MeWinCell<P>& c, int mylvl, int k, int px, int py);
-// Whether a context's star can start outside its range (see me_star_pattern): the global-memory contexts can; the
-// shared-memory windows only ever hold in-range starts (k_me_window hands the others to the global-memory kernel).
-template <typename CTX> struct MeStarFromOutside { static constexpr bool value = true; };
-template <typename P> struct MeStarFromOutside<MeWin<P> > { static constexpr bool value = false; };
-template <typename P> struct MeStarFromOutside<MeWinCell<P> > { static constexpr bool value = false; };
-
+// Two compile-time properties of the search contexts steer me_star_pattern: CTX::startsOutside (the star can start outside
+// its range; see below) and CTX::hasStarTable (the first star round of the PUs that start at the cell's common point reads
+// its candidates' SADs from a table computed once per 16x16 cell: me_star_lookup, me_window.cuh).
 template <typename CTX>
 __device__ __forceinline__ void me_star_pattern(const CTX& c, MeStar& s, int earlyExitIters, int merange, bool first = false)
 {
@@ -892,7 +877,7 @@ __device__ __forceinline__ void me_star_pattern(const CTX& c, MeStar& s, int ear
     // 548-589).  That is the range widened to include the start: the range itself when the start lies inside it.  The
     // start can lie outside it in x when MV 0 won the pre-checks (motion.cpp:787-796); then a point such as (ox, top) is
     // evaluated although ox is out of range.  Contexts that only see in-range starts keep the plain range.
-    constexpr bool OUT = MeStarFromOutside<CTX>::value;
+    constexpr bool OUT = CTX::startsOutside;
     const int lox = OUT ? min(c.minx, ox) : c.minx, hix = OUT ? max(c.maxx, ox) : c.maxx;
     const int loy = OUT ? min(c.miny, oy) : c.miny, hiy = OUT ? max(c.maxy, oy) : c.maxy;
     const bool spec = c.pow2 && c.nw <= 64;
@@ -914,8 +899,11 @@ __device__ __forceinline__ void me_star_pattern(const CTX& c, MeStar& s, int ear
         if (!valid) { px = min(max(ox, lox), hix); py = min(max(oy, loy), hiy); }
         const int n = spec ? (lvl0 == 0 ? 28 : 32) : (lvl0 == 0 ? 4 : lvl0 < 4 ? 8 : 16);
         // the first round of a cell's PUs that share the start point: SADs out of the cell's star table (me_window.cuh)
-        const int cost = (first && me_star_cached(c)) ? (valid ? me_star_lookup(c, mylvl, k, px, py) : 0x7fffffff)
-                                                      : me_eval_points(c, n, px, py, false);
+        int cost;
+        if constexpr (CTX::hasStarTable)
+            cost = (first && c.star) ? (valid ? me_star_lookup(c, mylvl, k, px, py) : 0x7fffffff) : me_eval_points(c, n, px, py, false);
+        else
+            cost = me_eval_points(c, n, px, py, false);
         for (int l = lvl0; l < lvl1; l++)
         {
             if (l >= 4 && (16 << (l - 4)) > merange) return;

@@ -51,12 +51,15 @@ struct MeWin
     bool pow2; int nw, lgnw, lgwpr, lgsegw;
     const struct MewCell* cell;            // shared 4x4 SAD maps of the 16x16 cell (NULL: this job walks its own raster)
     bool star;                             // this job starts at the cell's common start point: first star round out of the star table
+    // only in-range starts: k_me_window hands the others to the global-memory kernel
+    static constexpr bool startsOutside = false;
+    static constexpr bool hasStarTable = false;
 };
 
-// The context of the 16x16-cell kernel: same fields, its own overloads of me_raster / me_star_cached so that each kernel
+// The context of the 16x16-cell kernel: same fields, its own me_raster overload and the star table, so that each kernel
 // instantiation carries only the code it can execute (the kernels are instruction-cache bound: the CU 32 / CU 64 kernel has
 // no map / star-table code, the cell kernel none of the wide column-walk variants).
-template <typename P> struct MeWinCell : MeWin<P> {};
+template <typename P> struct MeWinCell : MeWin<P> { static constexpr bool hasStarTable = true; };
 
 // 16x16 cell groups: all PUs of the cell (16x16 CU + four 8x8 CUs) that share one raster grid (same mvmin / mvmax: the
 // predictor field is 16x16-granular, so inside the picture they all do) get their raster costs from ONE set of SAD maps:
@@ -88,6 +91,7 @@ __device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile
 __device__ __forceinline__ uint2 lds64(uint32_t a) { uint2 v; asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a)); return v; }
 __device__ __forceinline__ uint32_t lds16(uint32_t a) { uint32_t v; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ void sts16(uint32_t a, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void sts64(uint32_t a, uint2 v) { asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(a), "r"(v.x), "r"(v.y) : "memory"); }
 __device__ __forceinline__ uint4 lds128(uint32_t a) { uint4 v; asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; }
 
 // SEGW words of a window row starting at a byte address of any phase: SEGW + 1 aligned LDS.32 + SEGW funnel shifts.
@@ -195,8 +199,27 @@ __device__ __forceinline__ int me_eval_points(const MeWin<P>& c, int n, int px, 
 }
 // ---- raster refinement out of the window (motion.cpp:1171-1201) ---------------------------------------------------
 // Grid of step 5 over [minx, maxx] x [miny, maxy] in raster order; the reference's sequential `cost < bcost` chain = the
-// minimum with ties to the lowest raster index.  Lane = grid column; NA = accumulators = ceil(h / 5) (template: 2/4/7/13).
-template <typename P, int NA, int LGSEGW>
+// minimum with ties to the lowest raster index.  Each lane brings its best (cost, raster index); the grid's winner is the
+// warp's minimum cost, then the lowest index among the lanes that reach it.
+__device__ __forceinline__ void mew_grid_fold(int best, int bestIdx, int ncols, int minx, int miny, MeStar& s)
+{
+    const int m = __reduce_min_sync(0xffffffffu, best);
+    const int mi = __reduce_min_sync(0xffffffffu, best == m ? bestIdx : 0x7fffffff);
+    if (m < s.bcost)
+    {
+        s.bcost = m;
+        const int rj = mi / ncols, ri = mi - rj * ncols;
+        s.bx = minx + ri * 5; s.by = miny + rj * 5;
+    }
+}
+
+// Column walk: lane = grid column; NA = accumulators = ceil(h / 5) (template: 2/4/7/13).  Row policy:
+//   NSEG = 0: the row in SEGW-word segments, each loaded once and differenced against every live ring slot whose source row
+//             exists (a test per slot and segment);
+//   NSEG = 1, 2, 4: PUs whose rows are NSEG aligned 16-byte segments (LGSEGW = 2): the lane's whole reference row is loaded
+//             once into registers, then every live candidate (one bound per row) differences its source row against it,
+//             NSEG x (broadcast LDS.128 + 4 VABSDIFF4) with no per-segment conditions.
+template <typename P, int NA, int LGSEGW, int NSEG>
 __device__ __forceinline__ void mew_raster_t(const MeWin<P>& c, MeStar& s)
 {
     constexpr int SEGW = 1 << LGSEGW, SEGB = 4 * SEGW, RD = 5;
@@ -222,28 +245,50 @@ __device__ __forceinline__ void mew_raster_t(const MeWin<P>& c, MeStar& s)
         {
             const int lo = max(0, b - nrows + 1), hi = min(b, NA - 1);     // live ring slots: candidate k = b - i in [0, nrows)
 #pragma unroll 1
-            for (int t = 0; t < RD; t++)                                   // a loop, not unrolled: only the ring index i must be static
+            for (int t = 0; t < RD; t++, rowaddr += c.pitch)              // a loop, not unrolled: only the ring index i must be static
             {
-                if (b * RD + t <= lastRow)                                 // warp-uniform
+                if (b * RD + t > lastRow) continue;                        // warp-uniform
+                const uint32_t fa = c.fenc + t * c.fpitch;
+                if constexpr (NSEG > 0)
+                {
+                    uint32_t r[4 * NSEG];
+                    mew_load_ref<4 * NSEG>(rowaddr, sh, r);
+                    // slot i is live iff lo <= i <= hi and its source row 5 i + t exists
+                    const int ihi = c.h - 1 - t >= 0 ? min(hi, (c.h - 1 - t) / RD) : -1;
+#pragma unroll
+                    for (int i = 0; i < NA; i++)
+                    {
+                        if (i >= lo && i <= ihi)                           // warp-uniform
+                        {
+#pragma unroll
+                            for (int sg = 0; sg < NSEG; sg++)
+                            {
+                                uint32_t f[4];
+                                mew_load_fenc<4>(fa + (RD * i) * c.fpitch + sg * 16, f);     // same address in every lane: broadcast
+                                const uint32_t rw[4] = { r[4 * sg], r[4 * sg + 1], r[4 * sg + 2], r[4 * sg + 3] };
+                                acc[i] = sad_words<P, 4>(f, rw, acc[i]);
+                            }
+                        }
+                    }
+                }
+                else
                 {
                     for (int sg = 0; sg < nseg; sg++)
                     {
                         uint32_t r[SEGW];
                         mew_load_ref<SEGW>(rowaddr + sg * SEGB, sh, r);
-                        const uint32_t fa = c.fenc + t * c.fpitch + sg * SEGB;
 #pragma unroll
                         for (int i = 0; i < NA; i++)
                         {
                             if (i >= lo && i <= hi && RD * i + t < c.h)    // warp-uniform
                             {
                                 uint32_t f[SEGW];
-                                mew_load_fenc<SEGW>(fa + (RD * i) * c.fpitch, f);    // same address in every lane: broadcast
+                                mew_load_fenc<SEGW>(fa + sg * SEGB + (RD * i) * c.fpitch, f);    // same address in every lane: broadcast
                                 acc[i] = sad_words<P, SEGW>(f, r, acc[i]);
                             }
                         }
                     }
                 }
-                rowaddr += c.pitch;
             }
             const int k = b - (NA - 1);                                    // the candidate in the last ring slot is complete
             if (k >= 0)
@@ -258,120 +303,54 @@ __device__ __forceinline__ void mew_raster_t(const MeWin<P>& c, MeStar& s)
             acc[0] = 0;
         }
     }
-    const int m = __reduce_min_sync(0xffffffffu, best);
-    const int mi = __reduce_min_sync(0xffffffffu, best == m ? bestIdx : 0x7fffffff);
-    if (m < s.bcost)
-    {
-        s.bcost = m;
-        const int rj = mi / ncols, ri = mi - rj * ncols;
-        s.bx = c.minx + ri * RD; s.by = c.miny + rj * RD;
-    }
+    mew_grid_fold(best, bestIdx, ncols, c.minx, c.miny, s);
 }
 
-// The same column walk for PUs whose rows are 1, 2 or 4 aligned 16-byte segments (NSEG): the lane's whole reference row is
-// loaded once into registers, then every live candidate of the ring differences its source row against it -- per
-// (candidate, row): one liveness test, then NSEG x (broadcast LDS.128 + 4 VABSDIFF4), no per-segment conditions.
-template <typename P, int NA, int NSEG>
-__device__ __forceinline__ void mew_raster_wide(const MeWin<P>& c, MeStar& s)
-{
-    constexpr int RD = 5, NW = 4 * NSEG;
-    const int ncols = (c.maxx - c.minx) / RD + 1, nrows = (c.maxy - c.miny) / RD + 1;
-    const int lastRow = (nrows - 1) * RD + c.h - 1;
-    const int nblk = nrows + NA - 1;
-    int best = 0x7fffffff, bestIdx = 0x7fffffff;
-    for (int cbase = 0; cbase < ncols; cbase += 32)
-    {
-        const int ri = cbase + c.lane;
-        const bool act = ri < ncols;
-        const int cx = c.minx + (act ? ri : 0) * RD;
-        const bool x8 = (ri & 3) == 3;
-        const int xc = (int)__ldg(c.mvc + ((x8 ? cx * 8 : cx * 4) - c.mvpx));
-        const int ymul = x8 ? 8 : 4;
-        const uint32_t a0 = c.win + (uint32_t)((c.oy + c.miny) * c.pitch + (c.ox + cx) * (int)sizeof(P));
-        const unsigned sh = (a0 & 3u) * 8u;
-        uint32_t rowaddr = a0 & ~3u;
-        int acc[NA];
-#pragma unroll
-        for (int i = 0; i < NA; i++) acc[i] = 0;
-        for (int b = 0; b < nblk; b++)
-        {
-            const int lo = max(0, b - nrows + 1), hi = min(b, NA - 1);     // live ring slots: candidate k = b - i in [0, nrows)
-#pragma unroll 1
-            for (int t = 0; t < RD; t++, rowaddr += c.pitch)
-            {
-                if (b * RD + t > lastRow) continue;                        // warp-uniform
-                uint32_t w[NW + 1], r[NW];
-#pragma unroll
-                for (int q = 0; q <= NW; q++) w[q] = lds32(rowaddr + 4 * q);
-#pragma unroll
-                for (int q = 0; q < NW; q++) r[q] = __funnelshift_r(w[q], w[q + 1], sh);
-                // live candidates of this row: slot i is live iff lo <= i <= hi and its source row 5 i + t exists
-                const int ihi = c.h - 1 - t >= 0 ? min(hi, (c.h - 1 - t) / RD) : -1;
-                const uint32_t fa = c.fenc + t * c.fpitch;
-#pragma unroll
-                for (int i = 0; i < NA; i++)
-                {
-                    if (i >= lo && i <= ihi)                               // warp-uniform
-                    {
-#pragma unroll
-                        for (int sg = 0; sg < NSEG; sg++)
-                        {
-                            const uint4 f = lds128(fa + (RD * i) * c.fpitch + sg * 16);    // same address in every lane: broadcast
-                            const uint32_t fw[4] = { f.x, f.y, f.z, f.w };
-                            const uint32_t rw[4] = { r[4 * sg], r[4 * sg + 1], r[4 * sg + 2], r[4 * sg + 3] };
-                            acc[i] = sad_words<P, 4>(fw, rw, acc[i]);
-                        }
-                    }
-                }
-            }
-            const int k = b - (NA - 1);                                    // the candidate in the last ring slot is complete
-            if (k >= 0)
-            {
-                const int py = c.miny + k * RD;
-                const int cost = acc[NA - 1] + (int)(uint16_t)(xc + (int)__ldg(c.mvc + (py * ymul - c.mvpy)));
-                const int idx = k * ncols + ri;
-                if (act && (cost < best || (cost == best && idx < bestIdx))) { best = cost; bestIdx = idx; }
-            }
-#pragma unroll
-            for (int i = NA - 1; i > 0; i--) acc[i] = acc[i - 1];
-            acc[0] = 0;
-        }
-    }
-    const int m = __reduce_min_sync(0xffffffffu, best);
-    const int mi = __reduce_min_sync(0xffffffffu, best == m ? bestIdx : 0x7fffffff);
-    if (m < s.bcost)
-    {
-        s.bcost = m;
-        const int rj = mi / ncols, ri = mi - rj * ncols;
-        s.bx = c.minx + ri * RD; s.by = c.miny + rj * RD;
-    }
-}
-
-template <typename P, int NSEG>
-__device__ __forceinline__ void mew_raster_wide_na(const MeWin<P>& c, MeStar& s)
-{
-    if (c.h <= 10)      mew_raster_wide<P, 2, NSEG>(c, s);
-    else if (c.h <= 20) mew_raster_wide<P, 4, NSEG>(c, s);
-    else if (c.h <= 35) mew_raster_wide<P, 7, NSEG>(c, s);
-    else                mew_raster_wide<P, 13, NSEG>(c, s);
-}
-
-template <typename P, int LGSEGW>
+template <typename P, int LGSEGW, int NSEG>
 __device__ __forceinline__ void mew_raster_na(const MeWin<P>& c, MeStar& s)
 {
-    if (c.h <= 10)      mew_raster_t<P, 2, LGSEGW>(c, s);
-    else if (c.h <= 20) mew_raster_t<P, 4, LGSEGW>(c, s);
-    else if (c.h <= 35) mew_raster_t<P, 7, LGSEGW>(c, s);
-    else                mew_raster_t<P, 13, LGSEGW>(c, s);
+    if (c.h <= 10)      mew_raster_t<P, 2, LGSEGW, NSEG>(c, s);
+    else if (c.h <= 20) mew_raster_t<P, 4, LGSEGW, NSEG>(c, s);
+    else if (c.h <= 35) mew_raster_t<P, 7, LGSEGW, NSEG>(c, s);
+    else                mew_raster_t<P, 13, LGSEGW, NSEG>(c, s);
+}
+
+// One entry of the cell maps and of the star table: the SADs S[bx] of the four 4x4 blocks of a 16-pixel span over four rows
+// (window rows from `a4` at byte phase `sh`, row pitch `pitch`; source rows from `fa`, pitch 64 pixels), stored as the 4
+// prefix sums over the block columns, P[bx] = S[0] + .. + S[bx], as 4 x u16 in one 8-byte word (4 blocks of 16 ten-bit
+// pixels: <= 65472), so that a PU's block-row sum is P[last] - P[first - 1].
+template <typename P>
+__device__ __forceinline__ uint2 mew_block_row_prefix(uint32_t a4, unsigned sh, int pitch, uint32_t fa)
+{
+    constexpr int ES = (int)sizeof(P), WB = ES;                    // words per 4-pixel block row
+    int acc[4] = { 0, 0, 0, 0 };
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+    {
+#pragma unroll
+        for (int hw = 0; hw < WB; hw++)                            // 16 bytes of the row per step: 4 (8-bit) / 2 (16-bit) blocks
+        {
+            uint32_t rr[4], ff[4];
+            mew_load_ref<4>(a4 + r * pitch + hw * 16, sh, rr);
+            mew_load_fenc<4>(fa + r * 64 * ES + hw * 16, ff);      // same address in every lane of a map task: broadcast
+#pragma unroll
+            for (int wd = 0; wd < 4; wd++)
+            {
+                const int bx = (hw * 4 + wd) / WB;                 // block column of this word
+                acc[bx] = sad_word<P>(ff[wd], rr[wd], acc[bx]);
+            }
+        }
+    }
+    const uint32_t p0 = (uint32_t)acc[0], p1 = p0 + (uint32_t)acc[1], p2 = p1 + (uint32_t)acc[2], p3 = p2 + (uint32_t)acc[3];
+    return make_uint2(p0 | (p1 << 16), p2 | (p3 << 16));
 }
 
 // One task of the cell maps: grid row k, every grid column (lane = column), the cell's 4 block rows one after the other.
-// Stored per (block row, k, column): the 4 prefix sums over the block columns, P[bx] = S[0] + .. + S[bx], as 4 x u16 in
-// one 8-byte word (4 blocks of 16 ten-bit pixels: <= 65472), so that a PU's block-row sum is P[last] - P[first - 1].
+// Stored per (block row, k, column).
 template <typename P>
 __device__ __forceinline__ void mew_cell_map_task(const MeWin<P>& c, const MewCell& cell, int k)
 {
-    constexpr int ES = (int)sizeof(P), WB = ES;                    // words per 4-pixel block row
+    constexpr int ES = (int)sizeof(P);
     const int col = c.lane;
     const bool act = col < cell.ncols;
     const int gx = cell.minx + (act ? col : 0) * 5, gy = cell.miny + k * 5;
@@ -382,28 +361,8 @@ __device__ __forceinline__ void mew_cell_map_task(const MeWin<P>& c, const MewCe
 #pragma unroll 1
     for (int by = 0; by < 4; by++)
     {
-        int acc[4] = { 0, 0, 0, 0 };
-#pragma unroll
-        for (int r = 0; r < 4; r++)
-        {
-#pragma unroll
-            for (int hw = 0; hw < WB; hw++)                        // 16 bytes of the row per step: 4 (8-bit) / 2 (16-bit) blocks
-            {
-                uint32_t rr[4], ff[4];
-                mew_load_ref<4>(a4 + r * c.pitch + hw * 16, sh, rr);
-                mew_load_fenc<4>(fa + r * 64 * ES + hw * 16, ff);  // same address in every lane: broadcast
-#pragma unroll
-                for (int wd = 0; wd < 4; wd++)
-                {
-                    const int bx = (hw * 4 + wd) / WB;             // block column of this word
-                    acc[bx] = sad_word<P>(ff[wd], rr[wd], acc[bx]);
-                }
-            }
-        }
-        const uint32_t p0 = (uint32_t)acc[0], p1 = p0 + (uint32_t)acc[1], p2 = p1 + (uint32_t)acc[2], p3 = p2 + (uint32_t)acc[3];
-        if (act)
-            asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(cell.map + (uint32_t)(((by * MEW_MAP_ROWS + k) * 32 + col) * 8)),
-                         "r"(p0 | (p1 << 16)), "r"(p2 | (p3 << 16)) : "memory");
+        const uint2 v = mew_block_row_prefix<P>(a4, sh, c.pitch, fa);
+        if (act) sts64(cell.map + (uint32_t)(((by * MEW_MAP_ROWS + k) * 32 + col) * 8), v);
         a4 += 4 * c.pitch; fa += 4 * 64 * ES;
     }
 }
@@ -472,15 +431,7 @@ __device__ __forceinline__ void mew_raster_maps(const MeWin<P>& c, MeStar& s)
     else if (nby == 1) mew_maps_scan<1>(base, nrows, eoff, esh, soff, ssh, sx >= 0, cell->zero, xc, yp, ystep, best, bestRow);
     else               mew_maps_scan<3>(base, nrows, eoff, esh, soff, ssh, sx >= 0, cell->zero, xc, yp, ystep, best, bestRow);   // AMP: 12 rows
     if (!act) best = 0x7fffffff;
-    const int bestIdx = bestRow * ncols + col;
-    const int m = __reduce_min_sync(0xffffffffu, best);
-    const int mi = __reduce_min_sync(0xffffffffu, best == m ? bestIdx : 0x7fffffff);
-    if (m < s.bcost)
-    {
-        s.bcost = m;
-        const int rj = mi / ncols, ri = mi - rj * ncols;
-        s.bx = c.minx + ri * 5; s.by = c.miny + rj * 5;
-    }
+    mew_grid_fold(best, bestRow * ncols + col, ncols, c.minx, c.miny, s);
 }
 
 template <typename P>
@@ -488,12 +439,12 @@ __device__ __forceinline__ void me_raster(const MeWin<P>& c, MeStar& s)
 {
     // CU 32 / CU 64 groups.  pow2 PUs use the widest aligned segment; AMP widths (12 / 24 / 48) walk 4-byte words
     const int rowB = c.w * (int)sizeof(P);
-    if (c.pow2 && c.lgsegw == 2 && rowB == 64)      mew_raster_wide_na<P, 4>(c, s);
-    else if (c.pow2 && c.lgsegw == 2 && rowB == 32) mew_raster_wide_na<P, 2>(c, s);
-    else if (c.pow2 && c.lgsegw == 2 && rowB == 16) mew_raster_wide_na<P, 1>(c, s);
-    else if (c.pow2 && c.lgsegw == 2) mew_raster_na<P, 2>(c, s);
-    else if (c.pow2 && c.lgsegw == 1) mew_raster_na<P, 1>(c, s);
-    else                              mew_raster_na<P, 0>(c, s);
+    if (c.pow2 && c.lgsegw == 2 && rowB == 64)      mew_raster_na<P, 2, 4>(c, s);
+    else if (c.pow2 && c.lgsegw == 2 && rowB == 32) mew_raster_na<P, 2, 2>(c, s);
+    else if (c.pow2 && c.lgsegw == 2 && rowB == 16) mew_raster_na<P, 2, 1>(c, s);
+    else if (c.pow2 && c.lgsegw == 2) mew_raster_na<P, 2, 0>(c, s);
+    else if (c.pow2 && c.lgsegw == 1) mew_raster_na<P, 1, 0>(c, s);
+    else                              mew_raster_na<P, 0, 0>(c, s);
 }
 template <typename P>
 __device__ __forceinline__ void me_raster(const MeWinCell<P>& c, MeStar& s)
@@ -501,13 +452,10 @@ __device__ __forceinline__ void me_raster(const MeWinCell<P>& c, MeStar& s)
     // 16x16 cells: costs out of the shared SAD maps; a PU whose grid differs from the cell's (picture edges) walks its own
     // raster with the generic 4-byte-word variant
     if (c.cell) mew_raster_maps<P>(c, s);
-    else        mew_raster_na<P, 0>(c, s);
+    else        mew_raster_na<P, 0, 0>(c, s);
 }
 
 // First star round out of the cell's star table (me.cuh: me_star_pattern): candidate k of level `mylvl` around the common start.
-template <typename P> __device__ __forceinline__ bool me_star_cached(const MeWin<P>&) { return false; }
-template <typename P> __device__ __forceinline__ int me_star_lookup(const MeWin<P>&, int, int, int, int) { return 0; }
-template <typename P> __device__ __forceinline__ bool me_star_cached(const MeWinCell<P>& c) { return c.star; }
 template <typename P>
 __device__ __forceinline__ int me_star_lookup(const MeWinCell<P>& c, int mylvl, int k, int px, int py)
 {
@@ -530,7 +478,7 @@ __device__ __forceinline__ int me_star_lookup(const MeWinCell<P>& c, int mylvl, 
 template <typename P>
 __device__ __forceinline__ void mew_cell_star_build(const MewCell& cell, uint32_t win, int pitch, int tid)
 {
-    constexpr int ES = (int)sizeof(P), WB = ES;
+    constexpr int ES = (int)sizeof(P);
     const int idx = tid >> 2, by = tid & 3;
     if (idx >= MEW_STAR_POINTS) return;
     const int mylvl = idx < 4 ? 0 : idx < 28 ? 1 + ((idx - 4) >> 3) : 4 + ((idx - 28) >> 4);
@@ -539,25 +487,8 @@ __device__ __forceinline__ void mew_cell_star_build(const MewCell& cell, uint32_
     me_star_point(mylvl, k, cell.sx, cell.sy, px, py, point, dist);
     if (px < cell.minx || px > cell.maxx || py < cell.miny || py > cell.maxy) return;        // never looked up (out of the search range)
     const uint32_t a0 = win + (uint32_t)((cell.oy + py + 4 * by) * pitch + (cell.ox + px) * ES);
-    const unsigned sh = (a0 & 3u) * 8u;
-    const uint32_t a4 = a0 & ~3u;
     const uint32_t fa = cell.fenc + (uint32_t)(4 * by * 64 * ES);
-    int acc[4] = { 0, 0, 0, 0 };
-#pragma unroll
-    for (int r = 0; r < 4; r++)
-    {
-#pragma unroll
-        for (int hw = 0; hw < WB; hw++)
-        {
-            uint32_t rr[4], ff[4];
-            mew_load_ref<4>(a4 + r * pitch + hw * 16, sh, rr);
-            mew_load_fenc<4>(fa + r * 64 * ES + hw * 16, ff);
-#pragma unroll
-            for (int wd = 0; wd < 4; wd++) acc[(hw * 4 + wd) / WB] = sad_word<P>(ff[wd], rr[wd], acc[(hw * 4 + wd) / WB]);
-        }
-    }
-    const uint32_t p0 = (uint32_t)acc[0], p1 = p0 + (uint32_t)acc[1], p2 = p1 + (uint32_t)acc[2], p3 = p2 + (uint32_t)acc[3];
-    asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(cell.star + (uint32_t)((idx * 4 + by) * 8)), "r"(p0 | (p1 << 16)), "r"(p2 | (p3 << 16)) : "memory");
+    sts64(cell.star + (uint32_t)((idx * 4 + by) * 8), mew_block_row_prefix<P>(a0 & ~3u, (a0 & 3u) * 8u, pitch, fa));
 }
 
 // ---- mbarrier / TMA (PTX) -----------------------------------------------------------------------------------------
@@ -862,7 +793,6 @@ __global__ void __launch_bounds__(256) k_me_precheck_cell(const P* __restrict__ 
                                                           const MeGroup* __restrict__ groups, int ngroups, const int32_t* __restrict__ grp_jobs, int job0,
                                                           int cell, MeState* __restrict__ state, int* __restrict__ left_count, int32_t* __restrict__ left_list)
 {
-    constexpr int DEPTH = PixTraits<P>::depth;
     __shared__ __align__(16) MePreTab tabs[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int gi = blockIdx.x * 8 + warp;
@@ -905,43 +835,21 @@ __global__ void __launch_bounds__(256) k_me_precheck_cell(const P* __restrict__ 
         const int qy = k == 0 ? pmvy : k == 1 ? bmy * 4 : k == 2 ? 0 : k == 3 ? c0y : c1y;
         const int xf = qx & 3, yf = qy & 3;
         const P* r = rb + (qx >> 2) + (ptrdiff_t)(qy >> 2) * rstride;
-        int pr[8];
         if (xf && yf)
         {
             __syncwarp();
             for (int tk = lane; tk < (16 + 7) * 2; tk += 32)
             {
                 const int mrow = tk >> 1, sg = tk & 1;
-                int sum[8];
-                me_hrow<P, 8>(r + (ptrdiff_t)(mrow - 3) * rstride + sg * 8, xf, sum);
-                uint32_t pk[4];
-#pragma unroll
-                for (int i = 0; i < 4; i++)
-                    pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
-                *(uint4*)(t.mid + mrow * 16 + sg * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                me_hv_row<P, 8>(r + (ptrdiff_t)(mrow - 3) * rstride + sg * 8, xf, t.mid + mrow * 16 + sg * 8);
             }
             __syncwarp();
-            me_vmid<8>(t.mid + row * 16 + seg * 8, 16, yf, pr);
-#pragma unroll
-            for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 2);
         }
-        else
-        {
-            const P* rr = r + (ptrdiff_t)row * rstride + seg * 8;
-            if (!(xf | yf)) me_ld_px<P, 8>(rr, pr);
-            else if (!yf)
-            {
-                me_hrow<P, 8>(rr, xf, pr);
-#pragma unroll
-                for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 0);
-            }
-            else
-            {
-                me_vcol<P, 8>(rr - 3 * (ptrdiff_t)rstride, rstride, yf, pr);
-#pragma unroll
-                for (int x = 0; x < 8; x++) pr[x] = interp_finish<DEPTH>(pr[x], 0);
-            }
-        }
+        // full-pel rows as aligned words (me_ld_px): here they cost fewer instructions than me_pred_seg's scalar loads
+        const P* rr = r + (ptrdiff_t)row * rstride + seg * 8;
+        int pr[8];
+        if (!(xf | yf)) me_ld_px<P, 8>(rr, pr);
+        else me_pred_seg<P, 8, false>(rr, rstride, xf, yf, t.mid + row * 16 + seg * 8, 16, pr);
         int fv[8];
         me_ld_px<P, 8>(fb + (ptrdiff_t)row * fstride + seg * 8, fv);
         int sl = 0, sr = 0;

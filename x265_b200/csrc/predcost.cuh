@@ -229,7 +229,6 @@ __global__ void __launch_bounds__(128, TPJ == 32 ? 8 : 4) k_pred_cost(const P* _
 template <typename P, int NPX, bool SHORT>
 __device__ __forceinline__ void pb_seg(const MeCtx<P>& c, const P* __restrict__ ref, int qx, int qy, int (&pr)[NPX])
 {
-    constexpr int DEPTH = PixTraits<P>::depth;
     const int lane = c.lane;
     const int lgsegs = NPX == 8 ? c.lgw - 3 : 0, lgh = 31 - __clz(c.h);
     const int lpc = 1 << (lgh + lgsegs);
@@ -241,46 +240,13 @@ __device__ __forceinline__ void pb_seg(const MeCtx<P>& c, const P* __restrict__ 
         for (int t = lane; t < tasksPer; t += 32)
         {
             const int mrow = t >> lgsegs, seg = t & ((1 << lgsegs) - 1);
-            const P* s = ref + (qx >> 2) + (ptrdiff_t)((qy >> 2) - 3 + mrow) * c.rstride + seg * 8;
-            int sum[NPX];
-            me_hrow<P, NPX>(s, xf, sum);
-            uint32_t pk[NPX / 2];
-#pragma unroll
-            for (int i = 0; i < NPX / 2; i++)
-                pk[i] = ((uint32_t)interp_finish<DEPTH>(sum[2 * i], 1) & 0xffffu) | ((uint32_t)interp_finish<DEPTH>(sum[2 * i + 1], 1) << 16);
-            int16_t* d = mid + mrow * c.w + seg * 8;
-            if (NPX == 8) *(uint4*)d = make_uint4(pk[0], pk[1], pk[NPX / 2 - 2], pk[NPX / 2 - 1]);
-            else          *(uint2*)d = make_uint2(pk[0], pk[NPX / 2 - 1]);
+            me_hv_row<P, NPX>(ref + (qx >> 2) + (ptrdiff_t)((qy >> 2) - 3 + mrow) * c.rstride + seg * 8, xf, mid + mrow * c.w + seg * 8);
         }
     __syncwarp();
     const int sub = lane & (lpc - 1), row = sub & (c.h - 1), seg = sub >> lgh;
     if (lane < lpc)
-    {
-        const P* r = ref + (qx >> 2) + (ptrdiff_t)((qy >> 2) + row) * c.rstride + seg * 8;
-        if (!(xf | yf))
-        {
-#pragma unroll
-            for (int x = 0; x < NPX; x++) { const int p = (int)__ldg(r + x); pr[x] = SHORT ? (p << (14 - DEPTH)) - 8192 : p; }
-        }
-        else if (!yf)
-        {
-            me_hrow<P, NPX>(r, xf, pr);
-#pragma unroll
-            for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 1 : 0);
-        }
-        else if (!xf)
-        {
-            me_vcol<P, NPX>(r - 3 * (ptrdiff_t)c.rstride, c.rstride, yf, pr);
-#pragma unroll
-            for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 1 : 0);
-        }
-        else
-        {
-            me_vmid<NPX>(mid + row * c.w + seg * 8, c.w, yf, pr);
-#pragma unroll
-            for (int x = 0; x < NPX; x++) pr[x] = interp_finish<DEPTH>(pr[x], SHORT ? 3 : 2);
-        }
-    }
+        me_pred_seg<P, NPX, SHORT>(ref + (qx >> 2) + (ptrdiff_t)((qy >> 2) + row) * c.rstride + seg * 8, c.rstride, xf, yf,
+                                   mid + row * c.w + seg * 8, c.w, pr);
     else
     {
 #pragma unroll
@@ -319,36 +285,7 @@ __device__ __forceinline__ int pb_bi_luma(const MeCtx<P>& c, const P* __restrict
 #pragma unroll
         for (int x = 0; x < NPX; x++) d[x] = 0;
     }
-    int part = 0;
-    if (!satd)
-    {
-#pragma unroll
-        for (int x = 0; x < NPX; x++) part += abs(d[x]);
-        for (int o = 1; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    }
-    else
-    {
-#pragma unroll
-        for (int x = 0; x < NPX; x += 4) had4(d[x], d[x + 1], d[x + 2], d[x + 3]);
-#pragma unroll
-        for (int st = 1; st <= 2; st <<= 1)
-        {
-            const bool up = (lane & st) != 0;
-#pragma unroll
-            for (int x = 0; x < NPX; x++)
-            {
-                const int o = __shfl_xor_sync(0xffffffffu, d[x], st);
-                d[x] = up ? o - d[x] : o + d[x];
-            }
-        }
-#pragma unroll
-        for (int x = 0; x < NPX; x++) part += abs(d[x]);
-        part += __shfl_xor_sync(0xffffffffu, part, 1);
-        part += __shfl_xor_sync(0xffffffffu, part, 2);
-        part = (lane & 3) ? 0 : (part >> 1);                        // one 8x4 (4x4) tile per 4 lanes, halved per tile
-        for (int o = 4; o < lpc; o <<= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    }
-    return __shfl_sync(0xffffffffu, part, 0);
+    return __shfl_sync(0xffffffffu, me_seg_cost<NPX>(d, satd, lane, lpc), 0);
 }
 
 // Cb + Cr SATD of a bi-prediction's chroma (predInterChromaShort x 2 + addAvg), small PUs: me_chroma_batch_cols' lane mapping
