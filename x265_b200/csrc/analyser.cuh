@@ -38,6 +38,7 @@ struct x265cu_analyser
     // shared-memory-window integer search (me_window.cuh): group tables (two classes), tensor maps of the reference
     // planes [ref][MEW_NCLS], leftover list.  windowOn = 0 (X265CU_ME_WINDOW=0) keeps the global-memory kernel for all jobs.
     int windowOn; MeGroup* d_groups[3]; int32_t* d_grpJobs[3]; std::vector<int> rowGrp[3];
+    int cellJobsFit;                      // no 16x16 cell has more than 32 class-0 PUs (one lane each in k_me_subpel_cell)
     CUtensorMap* d_tmaps; int32_t* d_left;
     int32_t* d_order;                     // jobs of every CTU row sorted by PU shape (geometry.h)
     // quarter-pel phase planes of the sub-pel refinement (MePlanes, me.cuh): d_refs[r] is a block of 16 planes planeBytes
@@ -71,6 +72,18 @@ static void an_build_geometry(x265cu_analyser* a)
         a->d_groups[k] = an_upload(a->ctx, grp);
         a->d_grpJobs[k] = an_upload(a->ctx, g.grpJobs[k]);
         a->rowGrp[k].swap(g.rowGrp[k]);
+    }
+    // class-0 PUs (me_subpel_class: power-of-two sides of at most 16) per cell: at most 9 of the 16x16 CU + 5 per 8x8 CU
+    a->cellJobsFit = 1;
+    for (size_t i = 0; i < g.grpFirst[2].size(); i++)
+    {
+        int n = 0;
+        for (int q = g.grpFirst[2][i]; q < g.grpFirst[2][i] + g.grpCount[2][i]; q++)
+        {
+            const int w = a->pus[g.grpJobs[2][q]].pw, h = a->pus[g.grpJobs[2][q]].ph;
+            n += !((w & (w - 1)) | (h & (h - 1))) && w <= 16 && h <= 16;
+        }
+        if (n > 32) a->cellJobsFit = 0;
     }
 }
 
@@ -193,6 +206,8 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
             }
             win.job0 = job0; win.left_count = c->d_counter + 9; win.left_list = a->d_left;
             win.order = a->d_order + job0;
+            // workload[subme].hpel_satd (motion.cpp:48-58) is set from subme 2 on
+            win.subpelCells = a->p.subme >= 2 && a->cellJobsFit;
         }
         MePlanes pl;
         pl.nrefs = a->p.numRefs; pl.ppitch = (ptrdiff_t)(a->planeBytes / (depth == 8 ? 1 : 2));

@@ -1717,6 +1717,7 @@ struct MeWinLaunch
     int amp;                                                // AMP partitions present (13 PUs per CU instead of 5): sizes the CTAs
     const int32_t* order;                                   // the slice's jobs sorted by PU shape (absolute indices) or NULL
     int* left_count; int32_t* left_list;
+    int subpelCells;                                        // the class-0 sub-pel jobs of the cells run k_me_subpel_cell (hpel-SATD workloads)
 };
 template <typename P>
 static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, const uint16_t* mvcost, const x265cu_me_job* jobs,
@@ -1724,6 +1725,10 @@ static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, cons
 template <typename P>
 static int launch_me_precheck_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, const MeChromaArgs* ch,
                                      const uint16_t* mvcost, const x265cu_me_job* jobs, MeState* st, const MeWinLaunch& w, int* left_count, int32_t* left_list);
+template <typename P>
+static int launch_me_subpel_cells(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
+                                  const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
+                                  const MeWinLaunch& w);
 
 // Quarter-pel phase planes of the references (the frame analyser, analyser.cuh): every reference is one block of 16 planes
 // `ppitch` elements apart with the reference's stride and origin; slot yf * 4 + xf holds the luma plane interpolated at
@@ -1780,7 +1785,10 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
     // the phase planes are built inside the sub-pel phase, so its time includes them
     const ptrdiff_t pp = planes && !lowres ? planes->ppitch : 0;
     if (pp) rc |= me_build_planes<P>(ctx, *planes);
-    rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0, pp);
+    // every class-0 job belongs to a 16x16 cell (the CU 64 / CU 32 groups hold only class-1 PUs): with the cell kernel the
+    // per-PU class-0 launch has nothing left to do
+    if (grp && pp && win->subpelCells) rc |= launch_me_subpel_cells<P>(ctx, fenc, fstride, refs, rstride, pp, ch, mvcost, jobs, st, out, *win);
+    else rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0, pp);
     rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0, pp);
     return rc;
 }

@@ -947,6 +947,281 @@ __global__ void __launch_bounds__(256) k_me_precheck_cell(const P* __restrict__ 
     }
 }
 
+// ---- sub-pel refinement of the 16x16 cell groups (phase 3, motion.cpp:1440-1558) ---------------------------------------
+// What a candidate position yields does not depend on the PU that asks for it: the luma prediction at (qx, qy) is the
+// full-pel block of phase plane (qy & 3) * 4 + (qx & 3), the chroma prediction is fixed by the eighth-pel vector, and a PU's
+// SATD is the sum of its tiles -- 8x4 tiles (u_left + u_right) >> 1 for luma widths 8 and 16, 4x4 tiles u >> 1 for width 4,
+// u the un-halved 4x4 Hadamard sum (pixel.cpp:239-297); chroma as in k_me_precheck_cell.  So one warp runs the me_phase3
+// state machine of all small PUs of a cell (me_subpel_class 0: one lane per job, a cell has at most 29 of them) together,
+// and every step evaluates each distinct position the jobs ask for ONCE, over only the 8x4 luma units and chroma tiles that
+// the asking PUs cover.  Per job only the range test, mvcost and the arg-min remain.  The cell's 12-wide / 12-high AMP
+// parts (class 1) stay with the per-PU class-1 launch.  hpel-SATD workloads only (subme >= 2).
+#define MEC_NP 40                          // distinct positions per table fill; a step with more is evaluated in chunks
+struct MeSubTab
+{
+    int qx[MEC_NP], qy[MEC_NP];
+    int mask[MEC_NP];                      // bits 0-7: 8x4 luma units (tile row * 2 + 8-pixel column); 8-15: chroma tiles (plane * 4 + tile)
+    int start[MEC_NP];                     // exclusive prefix over the entries of the unit counts (bits 0-15) and tile counts (16-31)
+    int lum[MEC_NP][16];                   // un-halved luma 4x4 Hadamard sums, tile row * 4 + tile column
+    int chr[MEC_NP][8];                    // un-halved chroma 4x4 Hadamard sums [Cb tiles 0-3, Cr tiles 0-3]
+};
+
+// the entry of item `it` (0 <= it < total) of the 16-bit count field at `sh` of MeSubTab::start: the last entry starting at or
+// before it (which has a non-zero count)
+__device__ __forceinline__ int mec_find(const MeSubTab& t, int E, int it, int sh)
+{
+    int lo = 0, hi = E - 1;
+    while (lo < hi)
+    {
+        const int mid = (lo + hi + 1) >> 1;
+        if (((t.start[mid] >> sh) & 0xffff) <= it) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+template <typename P, bool CHROMA>
+__global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, ptrdiff_t ppitch,
+                                                        MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs,
+                                                        const MeGroup* __restrict__ groups, int ngroups, const int32_t* __restrict__ grp_jobs, int job0,
+                                                        const MeState* __restrict__ state, int32_t* __restrict__ out)
+{
+    __shared__ __align__(16) MeSubTab tabs[8];
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gi = blockIdx.x * 8 + warp;
+    if (gi >= ngroups) return;
+    const MeGroup g = groups[gi];
+    MeSubTab& t = tabs[warp];
+
+    // ---- the cell's class-0 jobs, one per lane, in group order (members lane and lane + 32: a cell holds up to 33 jobs) ----
+    int nj;
+    {
+        int m[2]; bool small[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+        {
+            const int i = lane + 32 * h;
+            m[h] = i < g.count ? grp_jobs[g.first + i] - job0 : 0;
+            const int pw = jobs[m[h]].pw, ph = jobs[m[h]].ph;
+            small[h] = i < g.count && !((pw & (pw - 1)) | (ph & (ph - 1))) && pw <= 16 && ph <= 16;
+        }
+        const unsigned b0 = __ballot_sync(FULL, small[0]), b1 = __ballot_sync(FULL, small[1]);
+        const unsigned lt = (1u << lane) - 1u;
+        // the analyser launches this kernel only when every cell has at most 32 of them (an_build_geometry)
+        if (small[0]) t.qx[__popc(b0 & lt)] = m[0];
+        if (small[1]) t.qx[__popc(b0) + __popc(b1 & lt)] = m[1];
+        nj = __popc(b0) + __popc(b1);
+    }
+    __syncwarp();
+    const bool mine = lane < nj;
+    const int jid = mine ? t.qx[lane] : grp_jobs[g.first] - job0;
+    __syncwarp();
+    const x265cu_me_job j = jobs[jid];
+    const int py = j.offset / fstride, px = j.offset - py * fstride;
+    const int cx = __shfl_sync(FULL, px, 0) & ~15, cy = __shfl_sync(FULL, py, 0) & ~15;
+    const ptrdiff_t coff = (ptrdiff_t)cy * fstride + cx;
+    const P* rb = refs[j.ref] + coff;                              // every job of a group has the same reference
+    const P* fb = fenc + coff;
+
+    // per job: its 4x4 tiles inside the cell, its units and chroma tiles, and me_phase3's start
+    const int bx0 = (px - cx) >> 2, by0 = (py - cy) >> 2, bw = j.pw >> 2, bh = j.ph >> 2;
+    const bool chromaOn = CHROMA && j.subme > 2 && !(j.pw & 7) && !(j.ph & 7);           // me_set_chroma
+    int mask = 0;
+    {
+        const int segs = (1 << (((bx0 + bw - 1) >> 1) + 1)) - (1 << (bx0 >> 1));
+        for (int y = by0; y < by0 + bh; y++) mask |= segs << (2 * y);
+        if (chromaOn)
+        {
+            const int tx0 = bx0 >> 1, ty0 = by0 >> 1, tw = j.pw >> 3, th = j.ph >> 3;
+            int cm = 0;
+            for (int y = ty0; y < ty0 + th; y++) for (int x = tx0; x < tx0 + tw; x++) cm |= 1 << (y * 2 + x);
+            mask |= (cm | (cm << 4)) << 8;
+        }
+    }
+    const int qminy = j.mvmin[1] * 4, qmaxy = j.mvmax[1] * 4, mvpx = j.qmvp[0], mvpy = j.qmvp[1];
+    const int8_t* wl = c_workload[j.subme];
+    const MeState st = state[jid];
+    int bcost = st.bcost, bx, by;
+    if (st.bprecost < bcost) { bx = st.bestprex; by = st.bestprey; bcost = st.bprecost; }
+    else { bx = st.bmx * 4; by = st.bmy * 4; }
+    bool live = mine && bcost != 0;
+    if (mine && !bcost) bcost = me_mvcost(mvcost, mvpx, mvpy, bx, by);
+    int stage = 0, it = 0;                                         // hpel SATD: stage 0 = SATD at the start point
+
+    for (;;)
+    {
+        if (live && stage == 1 && it >= wl[0]) { stage = 3; it = 0; }
+        if (live && stage == 3 && it >= wl[2]) live = false;
+        if (!__any_sync(FULL, live)) break;
+        const bool centre = stage == 0;
+        const int dirs = !live ? 0 : centre ? 1 : stage == 1 ? wl[1] : wl[3];
+        const int step = stage == 1 ? 2 : 1;
+        const int ndir = __reduce_max_sync(FULL, (unsigned)dirs);
+        unsigned sl0 = FULL, sl1 = FULL;                           // table entry of candidate i: byte i & 3 of (i < 4 ? sl0 : sl1)
+        int best = bcost, bdir = 0;
+        for (int i0 = 0; i0 < ndir;)
+        {
+            // ---- 1. requests of candidates i0 .. i1 - 1, deduplicated on (qx, qy), while the table has room ----
+            int E = 0, i1 = i0;
+            for (; i1 < ndir; i1++)
+            {
+                const int d1 = centre ? 0 : i1 + 1;
+                const int qx = bx + c_square1[d1][0] * step, qy = by + c_square1[d1][1] * step;
+                const bool have = i1 < dirs && (centre || !((qy < qminy) | (qy > qmaxy)));
+                const unsigned long long key = have ? ((unsigned long long)(uint32_t)qy << 32) | (uint32_t)qx : 0x8000000080000000ull;
+                const unsigned gm = __match_any_sync(FULL, key);
+                const int leader = __ffs(gm) - 1;
+                const bool lead = have && lane == leader;
+                int e = -1;
+                if (lead)
+                    for (int k = 0; k < E; k++) if (t.qx[k] == qx && t.qy[k] == qy) { e = k; break; }
+                const unsigned nb = __ballot_sync(FULL, lead && e < 0);
+                if (E + __popc(nb) > MEC_NP) break;                  // warp-uniform; E = 0 always has room
+                if (lead && e < 0) { e = E + __popc(nb & ((1u << lane) - 1u)); t.qx[e] = qx; t.qy[e] = qy; t.mask[e] = 0; }
+                E += __popc(nb);
+                e = __shfl_sync(FULL, e, leader);
+                __syncwarp();
+                if (have)
+                {
+                    atomicOr(&t.mask[e], mask);
+                    const unsigned sh = 8u * (i1 & 3), v = ((unsigned)e << sh) | ~(0xffu << sh);
+                    if (i1 < 4) sl0 &= v; else sl1 &= v;
+                }
+            }
+            __syncwarp();
+            // ---- 2. prefix of the entries' unit and tile counts ----
+            int total = 0;
+            for (int e0 = 0; e0 < E; e0 += 32)
+            {
+                const int e = e0 + lane;
+                const int m = e < E ? t.mask[e] : 0;
+                const int own = __popc(m & 0xff) | (__popc((m >> 8) & 0xff) << 16);
+                int v = own;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(FULL, v, o); if (lane >= o) v += n; }
+                if (e < E) t.start[e] = total + v - own;
+                total += __shfl_sync(FULL, v, 31);
+            }
+            __syncwarp();
+            // ---- 3. luma: 8 units per pass, a unit's 4 rows on 4 consecutive lanes (me_seg_cost's butterflies) ----
+            const int nu = total & 0xffff, nt = total >> 16;
+            for (int u0 = 0; u0 < nu; u0 += 8)
+            {
+                const int item = u0 + (lane >> 2), row = lane & 3;
+                const bool on = item < nu;
+                int e = 0, unit = 0;
+                int d[8];
+                if (on)
+                {
+                    e = mec_find(t, E, item, 0);
+                    unit = me_nth_set_bit((unsigned)t.mask[e] & 0xffu, item - (t.start[e] & 0xffff));
+                    const int qx = t.qx[e], qy = t.qy[e];
+                    const int y = (unit >> 1) * 4 + row, x = (unit & 1) * 8;
+                    int pr[8], fv[8];
+                    me_ld_px<P, 8>(rb + (qx >> 2) + (ptrdiff_t)((qy >> 2) + y) * rstride + x + ((qy & 3) * 4 + (qx & 3)) * ppitch, pr);
+                    me_ld_px<P, 8>(fb + (ptrdiff_t)y * fstride + x, fv);
+#pragma unroll
+                    for (int k = 0; k < 8; k++) d[k] = fv[k] - pr[k];
+                }
+                else
+                {
+#pragma unroll
+                    for (int k = 0; k < 8; k++) d[k] = 0;
+                }
+                had4(d[0], d[1], d[2], d[3]); had4(d[4], d[5], d[6], d[7]);
+#pragma unroll
+                for (int s = 1; s <= 2; s <<= 1)
+                {
+                    const bool up = (lane & s) != 0;
+#pragma unroll
+                    for (int k = 0; k < 8; k++)
+                    {
+                        const int o = __shfl_xor_sync(FULL, d[k], s);
+                        d[k] = up ? o - d[k] : o + d[k];
+                    }
+                }
+                int sl = abs(d[0]) + abs(d[1]) + abs(d[2]) + abs(d[3]), sr = abs(d[4]) + abs(d[5]) + abs(d[6]) + abs(d[7]);
+#pragma unroll
+                for (int s = 1; s <= 2; s <<= 1) { sl += __shfl_xor_sync(FULL, sl, s); sr += __shfl_xor_sync(FULL, sr, s); }
+                if (on && row == 0) { int* L = &t.lum[e][(unit >> 1) * 4 + (unit & 1) * 2]; L[0] = sl; L[1] = sr; }
+            }
+            // ---- 4. chroma: one lane per (position, plane, tile) ----
+            if (CHROMA)
+                for (int c0 = 0; c0 < nt; c0 += 32)
+                {
+                    const int item = c0 + lane;
+                    if (item < nt)
+                    {
+                        const int e = mec_find(t, E, item, 16);
+                        const int k = me_nth_set_bit(((unsigned)t.mask[e] >> 8) & 0xffu, item - (t.start[e] >> 16));
+                        const int cr = k >> 2, tt = k & 3, qx = t.qx[e], qy = t.qy[e];
+                        const ptrdiff_t o = (ptrdiff_t)(cy >> 1) * ch.cstride + (cx >> 1) + (ptrdiff_t)((tt >> 1) * 4) * ch.cstride + (tt & 1) * 4;
+                        const P* f = (const P*)(cr ? ch.fencCr : ch.fencCb) + o;
+                        const P* r = ((const P* const*)(cr ? ch.refCr : ch.refCb))[j.ref] + o + (qx >> 3) + (ptrdiff_t)(qy >> 3) * ch.cstride;
+                        t.chr[e][k] = me_chroma_had4x4<P>(f, r, ch.cstride, qx & 7, qy & 7);
+                    }
+                }
+            __syncwarp();
+            // ---- 5. each job folds its candidates i0 .. i1 - 1 in order (me_argmin: ties to the earliest) ----
+            for (int i = i0; i < i1; i++)
+            {
+                const int e = (int)(((i < 4 ? sl0 : sl1) >> (8 * (i & 3))) & 0xffu);
+                if (e == 0xff) continue;
+                const int d1 = centre ? 0 : i + 1;
+                const int qx = bx + c_square1[d1][0] * step, qy = by + c_square1[d1][1] * step;
+                const int* L = t.lum[e];
+                int cost = 0;
+                for (int y = by0; y < by0 + bh; y++)
+                {
+                    if (bw == 1) cost += L[y * 4 + bx0] >> 1;
+                    else for (int x = bx0; x < bx0 + bw; x += 2) cost += (L[y * 4 + x] + L[y * 4 + x + 1]) >> 1;
+                }
+                if (chromaOn)
+                {
+                    const int tx0 = bx0 >> 1, ty0 = by0 >> 1, th = j.ph >> 3;
+#pragma unroll
+                    for (int cr = 0; cr < 2; cr++)
+                        for (int y = ty0; y < ty0 + th; y++)
+                        {
+                            const int* s = &t.chr[e][cr * 4 + y * 2];
+                            cost += j.pw == 16 ? (s[0] + s[1]) >> 1 : s[tx0] >> 1;
+                        }
+                }
+                cost += me_mvcost(mvcost, mvpx, mvpy, qx, qy);
+                if (centre) best = cost;
+                else if (cost < best) { best = cost; bdir = d1; }
+            }
+            __syncwarp();
+            i0 = i1;
+        }
+        // ---- 6. the next stage, as me_phase3 ----
+        if (live)
+        {
+            if (centre) { bcost = best; stage = 1; }
+            else if (bdir) { bcost = best; bx += c_square1[bdir][0] * step; by += c_square1[bdir][1] * step; it++; }
+            else if (stage == 1) { stage = 3; it = 0; }
+            else live = false;
+        }
+    }
+    if (mine) { int32_t* o = out + (size_t)jid * 4; o[0] = bcost; o[1] = bx; o[2] = by; o[3] = 0; }
+}
+
+// Sub-pel refinement of the class-0 jobs of a frame slice's 16x16 cells (k_me_subpel_cell), on the phase planes `ppitch`
+// elements apart; the per-PU class-1 launch takes every other job.
+template <typename P>
+static int launch_me_subpel_cells(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
+                                  const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
+                                  const MeWinLaunch& w)
+{
+    if (w.ngroups[2] <= 0) return 0;
+    const MeChromaArgs none = {};
+    const auto kernel = ch ? k_me_subpel_cell<P, true> : k_me_subpel_cell<P, false>;
+    kernel<<<(w.ngroups[2] + 7) / 8, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ppitch, ch ? *ch : none, mvcost, jobs,
+                                                           (const MeGroup*)w.groups[2], w.ngroups[2], w.grp_jobs[2], w.job0, st, out);
+    CU_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
 // Pre-checks of a frame slice's groups: cells out of shared tables, every other job (CU 64 / CU 32 groups, cells' jobs with
 // other clips) appended to `left_list` (count in *left_count, zeroed here) for the per-PU kernels.
 template <typename P>
