@@ -218,7 +218,8 @@ int x265cu_pred_cost_batch(x265cu_ctx*, int depth, const void* fenc_dev, int fen
  * predictor field (AMVP / lowres MVs, search.cpp:1968-2023, 2406-2410) and gets back, for every PU x
  * reference, the motionEstimate() result (motion.cpp:739), for every CU the residual-coding stats of
  * its best 2Nx2N prediction (search.cpp:3178; quant.cpp:397-470, 543-605) and its 35 intra SA8D costs
- * (search.cpp:1358-1444).  stages: bit0 ME, bit1 residual, bit2 intra. */
+ * (search.cpp:1358-1444).  stages: bit0 ME, bit1 residual, bit2 intra, bit3 chroma residual (see
+ * x265cu_analyser_enable_chroma_residual). */
 typedef struct x265cu_analyser x265cu_analyser;
 typedef struct {
     int width, height, depth, numRefs;
@@ -273,6 +274,26 @@ int x265cu_analyser_set_ref_chroma(x265cu_analyser*, int idx, const void* cb_hos
 int x265cu_analyser_load_chroma(x265cu_analyser*, const void* cb_host, const void* cr_host, int host_stride);
 void* x265cu_analyser_recon_plane(x265cu_analyser*, int depthIdx /* 0..3 = CU 64,32,16,8 */, int* stride);
 int x265cu_analyser_recon_to_ref(x265cu_analyser*, int depthIdx, int refIdx, int ctuRow0, int ctuRow1);
+/* 4:2:0 chroma residual chain, stage bit 3 (value 8): for every CU, on the reference and vector the residual stage picks (lowest
+ * ME cost of the CU's 2Nx2N jobs, ties to the lowest index), and for each luma TU (T = min(S, 32)) one (T/2) x (T/2) TU per
+ * chroma plane at half the luma coordinates: predInterChromaPixel (predict.cpp:306-353) over the vector read as eighth-pel,
+ * sub_ps, dct, quant (flat lists, no RDOQ / sign hiding), dequant_normal, idct or the DC-only shortcut, add_ps with the
+ * recon clip, sse_pp (search.cpp:2990-3080).  The plane's quantiser QP is Quant::setChromaQP of qp - QP_BD_OFFSET + offset
+ * (quant.cpp:221-244).  Outputs: per CU and plane the SSE and the number of nonzero levels ([ncu][2]); per plane the levels
+ * (ncoef / 4: CU c's from its luma level offset / 4, TUs in the luma TU order); four recon planes per chroma plane, one per
+ * CU size, in the chroma geometry (stride / 2, margins 48 x 40).
+ * enable_chroma_residual() returns -1 (reason in x265cu_last_error) before enable_chroma() or for an offset outside -12..12
+ * (the HEVC range of the PPS + slice offset); a run with bit 3 returns -1 before any launch unless it has run. */
+int x265cu_analyser_enable_chroma_residual(x265cu_analyser*, int cbQpOffset, int crQpOffset);
+int x265cu_analyser_chroma_qp(x265cu_analyser*, int qp[2]);             /* quantiser QP of Cb, Cr */
+int x265cu_analyser_chroma_results(x265cu_analyser*, int ctuRow0, int ctuRow1, uint64_t* sse, uint32_t* numsig);
+                                                                       /* [ncu][2] full-frame host arrays, rows' slice filled */
+int x265cu_analyser_fetch_chroma(x265cu_analyser*, int what, void* host); /* 0 / 1: Cb / Cr levels; 2 + 2 * depthIdx + plane:
+                                                                          recon plane allocation; 10 + 2 * ref + plane: the
+                                                                          reference's chroma plane allocation */
+void* x265cu_analyser_recon_plane_chroma(x265cu_analyser*, int depthIdx, int plane, int* cstride);
+int x265cu_analyser_recon_to_ref_chroma(x265cu_analyser*, int depthIdx, int refIdx, int ctuRow0, int ctuRow1);
+int x265cu_analyser_ref_chroma_updated(x265cu_analyser*, int idx);     /* re-extend the chroma borders of ref idx */
 
 /* ---------- lookahead frame costs (BASELINE configs[1]; slicetype.cpp:696-805, 3115-3388) ----------
  * All pointers are device pointers.  Planes are the 4 lowres hpel planes of a frame (origin pixel,

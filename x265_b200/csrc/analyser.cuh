@@ -46,6 +46,12 @@ struct x265cu_analyser
     // phases, the same for every reference); per CTU row, the rectangle its sub-pel launches can read (AnRect below)
     x265cu_interp_job* d_planeJobs[3]; int nPlaneJobs[3];
     std::vector<int4> rowRead;
+    // 4:2:0 chroma residual stage (stage bit 3, x265cu_analyser_enable_chroma_residual): quantiser QP of Cb / Cr, levels of
+    // each plane (ncoef / 4), recon planes [depthIdx][plane] in the chroma geometry, per-CU [ncu][2] SSE / numSig
+    int chromaResOn, qpC[2];
+    int16_t* d_coefC[2]; uint8_t* d_reconC[4][2]; void** d_reconCTable;
+    unsigned long long* d_cu_sseC; uint32_t* d_cu_numsigC;
+    std::vector<GeoRect> rowReachC;       // per CTU row, the chroma pixels its chroma MC can read (geometry_chroma_reach)
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -165,6 +171,19 @@ static int an_build_plane_jobs(x265cu_analyser* a)
     return 0;
 }
 
+// the chroma MC of the CTU rows [r0, r1) reads inside the chroma plane allocations
+static bool an_chroma_reach_ok(const x265cu_analyser* a, int r0, int r1)
+{
+    GeoRect u = { 1 << 30, 1 << 30, -(1 << 30), -(1 << 30) };
+    for (int r = r0; r < r1; r++)
+    {
+        const GeoRect& g = a->rowReachC[r];
+        if (g.x0 > g.x1) continue;
+        u.x0 = min(u.x0, g.x0); u.y0 = min(u.y0, g.y0); u.x1 = max(u.x1, g.x1); u.y1 = max(u.y1, g.y1);
+    }
+    return geometry_chroma_reach_inside(u, a->p.width, a->p.height, a->cstride, AN_MARGIN_X / 2, AN_MARGIN_Y / 2);
+}
+
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
 // the intra table are indexed by the slice-local index inside the kernels, CU / TU records carry absolute indices.
 static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
@@ -173,6 +192,16 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     const int depth = a->p.depth;
     cudaSetDevice(c->device);
     if (r0 < 0 || r1 > a->ctuRows || r0 >= r1) { x265cu_set_error("analyser: bad CTU row range", cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    if ((stages & 8) && !(a->chromaOn && a->chromaResOn))
+    {
+        x265cu_set_error("analyser: stage bit 3 (chroma residual) needs x265cu_analyser_enable_chroma and _enable_chroma_residual", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    if ((stages & 8) && !an_chroma_reach_ok(a, r0, r1))
+    {
+        x265cu_set_error("analyser: the chroma planes do not cover what the chroma residual MC can read", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
     if ((stages & 1) && !an_planes_cover(a, r0, r1))
     {
         x265cu_set_error("analyser: the phase planes do not cover the rows the sub-pel search can read", cudaErrorInvalidValue, __FILE__, __LINE__);
@@ -246,6 +275,19 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         CU_LAUNCH_CHECK(c);
     }
     CU_CHECK(cudaEventRecord(a->ev[3], c->stream));
+    if ((stages & 8) && ntu > 0)
+    {
+        CU_CHECK(cudaMemsetAsync(a->d_cu_sseC + 2 * (size_t)cu0, 0, sizeof(unsigned long long) * 2 * ncu, c->stream));
+        CU_CHECK(cudaMemsetAsync(a->d_cu_numsigC + 2 * (size_t)cu0, 0, sizeof(uint32_t) * 2 * ncu, c->stream));
+        const void* fcb = a->d_fencC[0] + a->cOrgBytes; const void* fcr = a->d_fencC[1] + a->cOrgBytes;
+        if (depth == 8)
+            return launch_cu_chroma_residual<uint8_t>(c, fcb, fcr, a->d_refCbTable, a->d_refCrTable, a->cstride, a->d_cus, a->d_tus + tu0, ntu,
+                                                      a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->qpC[0], a->qpC[1], a->d_coefC[0], a->d_coefC[1],
+                                                      a->d_reconCTable, a->d_cu_sseC, a->d_cu_numsigC);
+        return launch_cu_chroma_residual<uint16_t>(c, fcb, fcr, a->d_refCbTable, a->d_refCrTable, a->cstride, a->d_cus, a->d_tus + tu0, ntu,
+                                                   a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->qpC[0], a->qpC[1], a->d_coefC[0], a->d_coefC[1],
+                                                   a->d_reconCTable, a->d_cu_sseC, a->d_cu_numsigC);
+    }
     return 0;
 }
 
@@ -320,6 +362,8 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     a->d_pus = an_upload(ctx, a->pus); a->d_cus = an_upload(ctx, a->cus); a->d_tus = an_upload(ctx, a->tus); a->d_cu_jobs = an_upload(ctx, a->cu_jobs);
     a->d_jobs = (x265cu_me_job*)x265cu_malloc(ctx, sizeof(x265cu_me_job) * a->njobs);
     a->d_me_out = (int32_t*)x265cu_malloc(ctx, sizeof(int32_t) * 4 * a->njobs);
+    // a residual stage run before any search reads vector 0 of every CU, which lies inside every plane's reach
+    if (a->d_me_out) cudaMemset(a->d_me_out, 0, sizeof(int32_t) * 4 * a->njobs);
     a->d_me_packed = (int2*)x265cu_malloc(ctx, sizeof(int2) * a->njobs);
     // shared-memory-window search: tensor maps over the reference plane allocations (STAR only; the other methods and any
     // group whose window does not fit go through the global-memory kernel)
@@ -381,6 +425,8 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     for (int d = 0; d < 4; d++) cudaFree(a->d_recon[d]);
     for (int k = 0; k < 2; k++) { cudaFree(a->d_fencC[k]); for (int r = 0; r < a->p.numRefs; r++) cudaFree(a->d_refC[r][k]); }
     cudaFree(a->d_refCbTable); cudaFree(a->d_refCrTable);
+    for (int k = 0; k < 2; k++) { cudaFree(a->d_coefC[k]); for (int d = 0; d < 4; d++) cudaFree(a->d_reconC[d][k]); }
+    cudaFree(a->d_reconCTable); cudaFree(a->d_cu_sseC); cudaFree(a->d_cu_numsigC);
     x265cu_host_free(a->h_fenc); x265cu_host_free(a->h_field);
     delete a;
 }
@@ -469,6 +515,124 @@ int x265cu_analyser_load_chroma(x265cu_analyser* a, const void* cb_host, const v
 {
     if (!a->chromaOn) return -1;
     if (an_upload_cplane(a, a->d_fencC[0], cb_host, host_stride) || an_upload_cplane(a, a->d_fencC[1], cr_host, host_stride)) return -1;
+    return 0;
+}
+
+// ---- 4:2:0 chroma residual chain (stage bit 3, chroma_resid.cuh) ----
+int x265cu_analyser_enable_chroma_residual(x265cu_analyser* a, int cbQpOffset, int crQpOffset)
+{
+    const char* bad = NULL;
+    if (!a->chromaOn) bad = "x265cu_analyser_enable_chroma_residual: chroma planes not enabled (x265cu_analyser_enable_chroma)";
+    // HEVC limits the PPS + slice chroma QP offset to -12..12; x265 checks the same range (param.cpp:1572-1575)
+    else if (cbQpOffset < -12 || cbQpOffset > 12 || crQpOffset < -12 || crQpOffset > 12)
+        bad = "x265cu_analyser_enable_chroma_residual: chroma QP offset outside -12..12";
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    x265cu_ctx* c = a->ctx;
+    cudaSetDevice(c->device);
+    a->qpC[0] = geometry_chroma_qp(a->p.qp, cbQpOffset, a->p.depth);
+    a->qpC[1] = geometry_chroma_qp(a->p.qp, crQpOffset, a->p.depth);
+    if (a->chromaResOn) return 0;
+    a->rowReachC.resize(a->ctuRows);
+    for (int r = 0; r < a->ctuRows; r++)
+        a->rowReachC[r] = geometry_chroma_reach(a->p.width, a->p.height, a->cus, a->tus, a->rowTu[r], a->rowTu[r + 1]);
+    if (!an_chroma_reach_ok(a, 0, a->ctuRows))
+    {
+        x265cu_set_error("x265cu_analyser_enable_chroma_residual: the chroma planes do not cover what the chroma MC can read", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    void* rect[8];
+    for (int k = 0; k < 2; k++)
+    {
+        a->d_coefC[k] = (int16_t*)x265cu_malloc(c, sizeof(int16_t) * (a->ncoef / 4) + 16);
+        if (!a->d_coefC[k]) return -1;
+        for (int d = 0; d < 4; d++)
+        {
+            a->d_reconC[d][k] = (uint8_t*)x265cu_malloc(c, a->cPlaneBytes);
+            if (!a->d_reconC[d][k]) return -1;
+            CU_CHECK(cudaMemset(a->d_reconC[d][k], 0, a->cPlaneBytes));
+            rect[2 * d + k] = a->d_reconC[d][k] + a->cOrgBytes;
+        }
+    }
+    a->d_reconCTable = (void**)x265cu_malloc(c, sizeof(void*) * 8);
+    a->d_cu_sseC = (unsigned long long*)x265cu_malloc(c, sizeof(unsigned long long) * 2 * a->ncu);
+    a->d_cu_numsigC = (uint32_t*)x265cu_malloc(c, sizeof(uint32_t) * 2 * a->ncu);
+    if (!a->d_reconCTable || !a->d_cu_sseC || !a->d_cu_numsigC) return -1;
+    CU_CHECK(cudaMemcpy(a->d_reconCTable, rect, sizeof(rect), cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemset(a->d_cu_sseC, 0, sizeof(unsigned long long) * 2 * a->ncu));
+    CU_CHECK(cudaMemset(a->d_cu_numsigC, 0, sizeof(uint32_t) * 2 * a->ncu));
+    a->chromaResOn = 1;
+    return 0;
+}
+
+// quantiser QP of Cb and Cr (Quant::setChromaQP, quant.cpp:221-244)
+int x265cu_analyser_chroma_qp(x265cu_analyser* a, int* qp2)
+{
+    if (!a->chromaResOn) return -1;
+    qp2[0] = a->qpC[0]; qp2[1] = a->qpC[1];
+    return 0;
+}
+
+// per-CU [cu][plane] SSE and numSig of the CTU rows [r0, r1) into full-frame sized host arrays (synchronous)
+int x265cu_analyser_chroma_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, uint64_t* sse, uint32_t* numsig)
+{
+    if (!a->chromaResOn || ctuRow0 < 0 || ctuRow1 > a->ctuRows || ctuRow0 > ctuRow1) return -1;
+    x265cu_ctx* c = a->ctx;
+    cudaSetDevice(c->device);
+    const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
+    if (sse && nc) CU_CHECK(cudaMemcpyAsync(sse + 2 * c0, a->d_cu_sseC + 2 * c0, sizeof(uint64_t) * 2 * nc, cudaMemcpyDeviceToHost, c->stream));
+    if (numsig && nc) CU_CHECK(cudaMemcpyAsync(numsig + 2 * c0, a->d_cu_numsigC + 2 * c0, sizeof(uint32_t) * 2 * nc, cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// what: 0 / 1 the Cb / Cr levels (ncoef / 4 each); 2 + 2 * depthIdx + plane the whole allocation of a chroma recon plane,
+// 10 + 2 * ref + plane the whole allocation of a reference's chroma plane (cstride x (height / 2 + 80) elements each)
+int x265cu_analyser_fetch_chroma(x265cu_analyser* a, int what, void* host)
+{
+    if (!a->chromaResOn || what < 0 || what >= 10 + 2 * a->p.numRefs) return -1;
+    x265cu_ctx* c = a->ctx;
+    const size_t es = a->p.depth == 8 ? 1 : 2, planeBytes = (size_t)a->cstride * a->cRows * es;
+    const void* src; size_t bytes;
+    if (what < 2) { src = a->d_coefC[what]; bytes = sizeof(int16_t) * (a->ncoef / 4); }
+    else if (what < 10) { src = a->d_reconC[(what - 2) >> 1][what & 1]; bytes = planeBytes; }
+    else { src = a->d_refC[(what - 10) >> 1][what & 1]; bytes = planeBytes; }
+    cudaSetDevice(c->device);
+    CU_CHECK(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// device address of the origin pixel of chroma recon plane (depthIdx, plane) and its stride in elements
+void* x265cu_analyser_recon_plane_chroma(x265cu_analyser* a, int depthIdx, int plane, int* cstride)
+{
+    if (!a->chromaResOn || depthIdx < 0 || depthIdx >= 4 || plane < 0 || plane > 1) return NULL;
+    *cstride = a->cstride;
+    return a->d_reconC[depthIdx][plane] + a->cOrgBytes;
+}
+
+// promote the chroma rows of CTU rows [ctuRow0, ctuRow1) of recon depth depthIdx (both planes) to reference idx; call
+// x265cu_analyser_ref_chroma_updated() once all rows of the new reference are in place
+int x265cu_analyser_recon_to_ref_chroma(x265cu_analyser* a, int depthIdx, int idx, int ctuRow0, int ctuRow1)
+{
+    if (!a->chromaResOn || depthIdx < 0 || depthIdx >= 4 || idx < 0 || idx >= a->p.numRefs || ctuRow0 < 0 || ctuRow1 > a->ctuRows || ctuRow0 >= ctuRow1) return -1;
+    const size_t es = a->p.depth == 8 ? 1 : 2;
+    const int ch = a->p.height >> 1, y0 = ctuRow0 * 32, y1 = ctuRow1 * 32 < ch ? ctuRow1 * 32 : ch;
+    cudaSetDevice(a->ctx->device);
+    const size_t off = a->cOrgBytes + (size_t)y0 * a->cstride * es, pitch = (size_t)a->cstride * es;
+    for (int k = 0; k < 2; k++)
+        CU_CHECK(cudaMemcpy2DAsync(a->d_refC[idx][k] + off, pitch, a->d_reconC[depthIdx][k] + off, pitch, (size_t)(a->p.width >> 1) * es, y1 - y0,
+                                   cudaMemcpyDeviceToDevice, a->ctx->stream));
+    return 0;
+}
+
+// re-extend the borders of reference idx's chroma planes (extendPicBorder with the chroma margins)
+int x265cu_analyser_ref_chroma_updated(x265cu_analyser* a, int idx)
+{
+    if (!a->chromaOn || idx < 0 || idx >= a->p.numRefs) return -1;
+    cudaSetDevice(a->ctx->device);
+    for (int k = 0; k < 2; k++)
+        if (x265cu_extend_border(a->ctx, a->p.depth, a->d_refC[idx][k] + a->cOrgBytes, a->cstride, a->p.width >> 1, a->p.height >> 1,
+                                 AN_MARGIN_X / 2, AN_MARGIN_Y / 2)) return -1;
     return 0;
 }
 

@@ -54,6 +54,74 @@ static inline int geometry_cu_parts(int size, int rect, int amp, int part[13][4]
     return n;
 }
 
+// ---- 4:2:0 chroma residual stage (analyser stage bit 3) ----
+#ifdef __CUDACC__
+#define GEO_HD __host__ __device__ __forceinline__
+#else
+#define GEO_HD inline
+#endif
+
+// The chroma TU of a luma TU (T = min(S, 32)): (T/2) x (T/2) at half the luma coordinates.  Its levels start at
+// coef_off / 4 + (TU index in the CU) * (T/2)^2, so each chroma plane holds ncoef / 4 levels in the luma TU order.
+struct ChromaTu { int x, y, size; int64_t off; };
+GEO_HD ChromaTu geometry_chroma_tu(const CuDesc& cu, const TuDesc& tu)
+{
+    const int S = cu.size, T = S > 32 ? 32 : S, Tc = T >> 1;
+    ChromaTu c;
+    c.x = (cu.x + tu.tx) >> 1; c.y = (cu.y + tu.ty) >> 1; c.size = Tc;
+    c.off = cu.coef_off / 4 + (int64_t)((tu.ty / T) * (S / T) + tu.tx / T) * Tc * Tc;
+    return c;
+}
+
+// Quant::setChromaQP (quant.cpp:221-244) for 4:2:0: qp is the analyser's quantiser QP (QP_BD_OFFSET included), offset the
+// plane's PPS + slice offset (-12..12).  Returns the plane's quantiser QP.
+static inline int geometry_chroma_qp(int qp, int offset, int depth)
+{
+    static const uint8_t chromaScale[58] = {                      // g_chromaScale (constants.cpp:346), entries 0..57
+        0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29,
+        29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37, 38, 39, 40, 41, 42, 43, 44, 45, 46, 47, 48, 49, 50, 51 };
+    const int bd = 6 * (depth - 8);
+    int q = qp - bd + offset;
+    q = q < -bd ? -bd : (q > 57 ? 57 : q);
+    if (q >= 30) q = chromaScale[q];
+    return q + bd;
+}
+
+// Chroma pixels (picture-relative, inclusive) that the chroma MC of the TUs [tu0, tu1) can read.  The vector of a CU is its
+// 2Nx2N PU's search result (or 0 before any search: the ME output is zeroed at creation).  The search clips with
+// k_build_me_jobs' rule, full-pel x in [-(71 + cuX), W + 7 - cuX] and y in [-(71 + cuY), H + 7 - cuY]; y stays inside that
+// range in quarter pels, x can leave it by 5 full pels below and 4 above plus the quarter-pel fraction (analyser.cuh, above
+// AN_PLANE_X).  The luma quarter-pel vector is the chroma eighth-pel vector; the 4-tap filter reads 1 pixel before and 2
+// after the block, and the kernel loads single pixels (no wider over-read).
+struct GeoRect { int x0, y0, x1, y1; };
+static inline int geo_floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+static inline GeoRect geometry_chroma_reach(int W, int H, const std::vector<CuDesc>& cus, const std::vector<TuDesc>& tus, int tu0, int tu1)
+{
+    GeoRect r = { 1 << 30, 1 << 30, -(1 << 30), -(1 << 30) };
+    for (int t = tu0; t < tu1; t++)
+    {
+        const CuDesc& cu = cus[tus[t].cu];
+        const ChromaTu c = geometry_chroma_tu(cu, tus[t]);
+        const int qxmin = 4 * (-(71 + cu.x) - 5), qxmax = 4 * (W + 7 - cu.x + 4) + 3;
+        const int qymin = 4 * (-(71 + cu.y)), qymax = 4 * (H + 7 - cu.y);
+        const int x0 = c.x + geo_floor_div(qxmin, 8) - 1, x1 = c.x + c.size - 1 + geo_floor_div(qxmax, 8) + 2;
+        const int y0 = c.y + geo_floor_div(qymin, 8) - 1, y1 = c.y + c.size - 1 + geo_floor_div(qymax, 8) + 2;
+        if (x0 < r.x0) r.x0 = x0;
+        if (y0 < r.y0) r.y0 = y0;
+        if (x1 > r.x1) r.x1 = x1;
+        if (y1 > r.y1) r.y1 = y1;
+    }
+    return r;
+}
+
+// The reach lies inside a chroma plane allocation of `cstride` elements per row with the picture origin at (mx, my) and
+// (H / 2 + 2 * my) rows
+static inline bool geometry_chroma_reach_inside(const GeoRect& r, int W, int H, int cstride, int mx, int my)
+{
+    if (r.x0 > r.x1) return true;                                  // no TU
+    return r.x0 >= -mx && r.x1 < cstride - mx && r.y0 >= -my && r.y1 < (H >> 1) + my && W / 2 + mx <= cstride;
+}
+
 static inline void geometry_build(int W, int H, int stride, int nref, int rect, int amp, FrameGeometry& g)
 {
     // CU list: CTU raster, sizes 64..8, raster inside the CTU; CUs must lie fully inside the picture

@@ -287,7 +287,15 @@ _AN_PROTOS = {
     "x265cu_analyser_enable_chroma": (I, [P]),
     "x265cu_analyser_set_ref_chroma": (I, [P, I, P, P, I]),
     "x265cu_analyser_load_chroma": (I, [P, P, P, I]),
+    "x265cu_analyser_enable_chroma_residual": (I, [P, I, I]),
+    "x265cu_analyser_chroma_qp": (I, [P, P]),
+    "x265cu_analyser_chroma_results": (I, [P, I, I, P, P]),
+    "x265cu_analyser_fetch_chroma": (I, [P, I, P]),
+    "x265cu_analyser_recon_plane_chroma": (P, [P, I, I, C.POINTER(I)]),
+    "x265cu_analyser_recon_to_ref_chroma": (I, [P, I, I, I, I]),
+    "x265cu_analyser_ref_chroma_updated": (I, [P, I]),
 }
+STAGE_CHROMA_RESIDUAL = 8                 # analyser stage bit 3 (x265cu_analyser_enable_chroma_residual)
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
 _AN_PROTOS["x265cu_lowres_intra_batch"] = (I, [P, I, P, I, I, I, I, I])
 _AN_PROTOS["x265cu_lookahead_cost_batch"] = (I, [P, I, P, I, I, I, I, P])
@@ -392,6 +400,56 @@ class Analyser:
         """Source chroma of the next analyse() / run_*() (pass pinned arrays for true async DMA)."""
         assert cb.shape == cr.shape == (self.height // 2, self.width // 2) and cb.dtype == self.dtype and cb.flags.c_contiguous and cr.flags.c_contiguous
         self.lib.check(self.lib.L.x265cu_analyser_load_chroma(self.h, cb.ctypes.data, cr.ctypes.data, self.width // 2))
+
+    # ---- 4:2:0 chroma residual chain (stage bit 3) ----
+    def enable_chroma_residual(self, cb_qp_offset=0, cr_qp_offset=0):
+        """Allocates the chroma residual outputs and sets the planes' QP offsets (PPS + slice, -12..12); needs
+        enable_chroma().  Afterwards runs may set stage bit 3 (STAGE_CHROMA_RESIDUAL)."""
+        self.lib.check(self.lib.L.x265cu_analyser_enable_chroma_residual(self.h, cb_qp_offset, cr_qp_offset))
+
+    def chroma_qp(self):
+        """(Cb, Cr) quantiser QPs of the chroma residual stage."""
+        q = (C.c_int * 2)()
+        self.lib.check(self.lib.L.x265cu_analyser_chroma_qp(self.h, q))
+        return q[0], q[1]
+
+    def chroma_results(self, r0=0, r1=None, sse=None, numsig=None):
+        """Per-CU [ncu][2] (Cb, Cr) SSE and number of nonzero levels of the CTU rows [r0, r1) (default: all), into the given
+        full-frame arrays or new zeroed ones; returns (sse, numsig)."""
+        r1 = self.ctu_rows if r1 is None else r1
+        sse = np.zeros((self.ncu, 2), np.uint64) if sse is None else sse
+        numsig = np.zeros((self.ncu, 2), np.uint32) if numsig is None else numsig
+        assert sse.shape == numsig.shape == (self.ncu, 2) and sse.dtype == np.uint64 and numsig.dtype == np.uint32
+        self.lib.check(self.lib.L.x265cu_analyser_chroma_results(self.h, r0, r1, sse.ctypes.data, numsig.ctypes.data))
+        return sse, numsig
+
+    def chroma_plane_shape(self):
+        """(rows, cstride) of a chroma plane allocation: the picture's origin is at row 40, column 48."""
+        return self.height // 2 + 80, self.stride // 2
+
+    def fetch_chroma(self, what):
+        """"coef_cb" / "coef_cr": a plane's levels (ncoef / 4); ("recon", depthIdx, plane): the whole allocation of a chroma
+        recon plane; ("ref", ref, plane): the whole allocation of a reference's chroma plane."""
+        if what in ("coef_cb", "coef_cr"):
+            out = np.zeros(self.ncoef // 4, np.int16)
+            idx = 0 if what == "coef_cb" else 1
+        else:
+            kind, a, plane = what
+            assert plane in (0, 1) and (kind == "recon" and 0 <= a < 4 or kind == "ref" and 0 <= a < self.numRefs), what
+            out = np.zeros(self.chroma_plane_shape(), self.dtype)
+            idx = (2 if kind == "recon" else 10) + 2 * a + plane
+        self.lib.check(self.lib.L.x265cu_analyser_fetch_chroma(self.h, idx, out.ctypes.data))
+        return out
+
+    def recon_plane_chroma_ptr(self, depth_idx, plane):
+        st = I()
+        return self.lib.L.x265cu_analyser_recon_plane_chroma(self.h, depth_idx, plane, C.byref(st)), st.value
+
+    def recon_to_ref_chroma(self, depth_idx, ref_idx, r0, r1):
+        self.lib.check(self.lib.L.x265cu_analyser_recon_to_ref_chroma(self.h, depth_idx, ref_idx, r0, r1))
+
+    def ref_chroma_updated(self, idx):
+        self.lib.check(self.lib.L.x265cu_analyser_ref_chroma_updated(self.h, idx))
 
     def h2d_bytes(self, field):
         return self.width * self.height * np.dtype(self.dtype).itemsize + field.nbytes
