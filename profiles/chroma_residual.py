@@ -1,7 +1,7 @@
-"""Device time of the frame analyser's 4:2:0 chroma residual stage (stage bit 3, chroma_resid.cuh) against the luma residual
-stage (bit 1, k_cu_residual) measured in the same call, at bench.py's c3 and c4 shapes.  ME runs once; then stage 2 and
-stage 8 are timed alternately with CUDA events (x265cu_timer_begin / _end around run_resident), after warm-up.  Reports the
-chroma stage's achieved bandwidth from its compulsory bytes (source and reference chroma read once per TU, levels and recon
+"""Device time of the frame analyser's 4:2:0 chroma residual stage (stage bit 3) against the luma residual stage (bit 1)
+measured in the same call, at bench.py's c3 and c4 shapes; both are instantiations of k_cu_residual (resid.cuh).  ME runs
+once; then stage 2 and stage 8 are timed alternately with CUDA events (x265cu_timer_begin / _end around run_resident), after
+warm-up.  Reports the chroma stage's achieved bandwidth from its compulsory bytes (source and reference chroma read once per TU, levels and recon
 written), with the card's name and power limit.  Needs a GPU; prints one JSON line per config.
 
     python profiles/chroma_residual.py [--configs c3,c4] [--reps 20] [--out DIR]

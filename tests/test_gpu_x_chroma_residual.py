@@ -1,4 +1,4 @@
-"""GPU parity of the frame analyser's 4:2:0 chroma residual stage (stage bit 3, x265_b200/csrc/chroma_resid.cuh) against the
+"""GPU parity of the frame analyser's 4:2:0 chroma residual stage (stage bit 3, x265_b200/csrc/resid.cuh) against the
 oracle's frame driver, which tests/test_chroma_residual_oracle_vs_ref.py pins to the real reference code: chroma levels, chroma
 recon planes and per-CU chroma SSE / numSig, with the luma outputs of the same run.  Row shards, promotion of the chroma recon
 to a reference, a second frame searched on the device-reconstructed references, and the refusals.  Kept in a file that sorts

@@ -1,6 +1,6 @@
-"""GPU parity of the frame analyser across the quantiser's QP range.  k_cu_residual keeps its own copy of the quantiser
-(the scale chains indexed by qp % 6, the shifts from qp / 6, the int16 clip of the levels, the DC-only shortcut and the
-clip of the reconstruction), and the mv cost lambda of each QP decides the searches: at QP 0 SAD ties do, at the top QP
+"""GPU parity of the frame analyser across the quantiser's QP range.  The residual chain of k_cu_residual has its own
+restatement of the quantiser (resid_quant's scale chains indexed by qp % 6 and shifts from qp / 6, the int16 clip of the
+levels, the DC-only shortcut and the clip of the reconstruction), and the mv cost lambda of each QP decides the searches: at QP 0 SAD ties do, at the top QP
 the MVP does.  Every case of test_frame_oracle_vs_ref.py::test_frame_driver_qp, which pins the oracle's frame driver to
 the reference on the same workloads, is compared bit for bit with that driver, with the same host-checked
 preconditions; at 512x320, where most search windows are away from the picture edge, the cut and the flat areas run

@@ -3,6 +3,7 @@
 #pragma once
 #include "common.cuh"
 #include "frame.cuh"
+#include "resid.cuh"
 #include "me.cuh"
 #include "me_window.cuh"
 #include <vector>
@@ -184,6 +185,28 @@ static bool an_chroma_reach_ok(const x265cu_analyser* a, int r0, int r1)
     return geometry_chroma_reach_inside(u, a->p.width, a->p.height, a->cstride, AN_MARGIN_X / 2, AN_MARGIN_Y / 2);
 }
 
+// the residual stage of the luma plane or of both 4:2:0 chroma planes over the CUs [cu0, cu0 + ncu) and their TUs
+static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int tu0, int ntu)
+{
+    x265cu_ctx* c = a->ctx;
+    const int npl = chroma ? 2 : 1;
+    ResidArgs r = {};
+    for (int p = 0; p < npl; p++)
+    {
+        r.fenc[p] = chroma ? a->d_fencC[p] + a->cOrgBytes : a->d_fenc + a->orgBytes;
+        r.refs[p] = chroma ? (p ? a->d_refCrTable : a->d_refCbTable) : a->d_refTable;
+        r.coef[p] = chroma ? a->d_coefC[p] : a->d_coef;
+        r.qp[p] = chroma ? a->qpC[p] : a->p.qp;
+    }
+    r.stride = chroma ? a->cstride : a->stride; r.recon = chroma ? a->d_reconCTable : a->d_reconTable;
+    r.cus = a->d_cus; r.tus = a->d_tus + tu0; r.ntu = ntu; r.cu_jobs = a->d_cu_jobs; r.numRefs = a->p.numRefs; r.me_out = a->d_me_out;
+    r.cu_sse = chroma ? a->d_cu_sseC : a->d_cu_sse; r.cu_numsig = chroma ? a->d_cu_numsigC : a->d_cu_numsig;
+    r.cu_ref = chroma ? NULL : a->d_cu_ref;
+    CU_CHECK(cudaMemsetAsync(r.cu_sse + (size_t)npl * cu0, 0, sizeof(unsigned long long) * npl * ncu, c->stream));
+    CU_CHECK(cudaMemsetAsync(r.cu_numsig + (size_t)npl * cu0, 0, sizeof(uint32_t) * npl * ncu, c->stream));
+    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r) : launch_resid<uint16_t>(c, chroma, r);
+}
+
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
 // the intra table are indexed by the slice-local index inside the kernels, CU / TU records carry absolute indices.
 static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
@@ -251,21 +274,7 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     }
     else if (stages & 1) CU_CHECK(cudaEventRecord(a->ev[4], c->stream));
     CU_CHECK(cudaEventRecord(a->ev[1], c->stream));
-    if ((stages & 2) && ntu > 0)
-    {
-        CU_CHECK(cudaMemsetAsync(a->d_cu_sse + cu0, 0, sizeof(unsigned long long) * ncu, c->stream));
-        CU_CHECK(cudaMemsetAsync(a->d_cu_numsig + cu0, 0, sizeof(uint32_t) * ncu, c->stream));
-        int blocks = ntu < c->sm_count * 8 ? ntu : c->sm_count * 8;
-        if (depth == 8)
-            k_cu_residual<uint8_t><<<blocks, 256, 0, c->stream>>>((const uint8_t*)(a->d_fenc + a->orgBytes), (const uint8_t* const*)a->d_refTable, a->stride,
-                a->d_cus, a->d_tus + tu0, ntu, a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->p.qp, a->d_coef, (uint8_t* const*)a->d_reconTable,
-                a->d_cu_sse, a->d_cu_numsig, a->d_cu_ref);
-        else
-            k_cu_residual<uint16_t><<<blocks, 256, 0, c->stream>>>((const uint16_t*)(a->d_fenc + a->orgBytes), (const uint16_t* const*)a->d_refTable, a->stride,
-                a->d_cus, a->d_tus + tu0, ntu, a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->p.qp, a->d_coef, (uint16_t* const*)a->d_reconTable,
-                a->d_cu_sse, a->d_cu_numsig, a->d_cu_ref);
-        CU_LAUNCH_CHECK(c);
-    }
+    if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, tu0, ntu)) return -1;
     CU_CHECK(cudaEventRecord(a->ev[2], c->stream));
     if ((stages & 4) && ncu > 0)
     {
@@ -275,19 +284,7 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         CU_LAUNCH_CHECK(c);
     }
     CU_CHECK(cudaEventRecord(a->ev[3], c->stream));
-    if ((stages & 8) && ntu > 0)
-    {
-        CU_CHECK(cudaMemsetAsync(a->d_cu_sseC + 2 * (size_t)cu0, 0, sizeof(unsigned long long) * 2 * ncu, c->stream));
-        CU_CHECK(cudaMemsetAsync(a->d_cu_numsigC + 2 * (size_t)cu0, 0, sizeof(uint32_t) * 2 * ncu, c->stream));
-        const void* fcb = a->d_fencC[0] + a->cOrgBytes; const void* fcr = a->d_fencC[1] + a->cOrgBytes;
-        if (depth == 8)
-            return launch_cu_chroma_residual<uint8_t>(c, fcb, fcr, a->d_refCbTable, a->d_refCrTable, a->cstride, a->d_cus, a->d_tus + tu0, ntu,
-                                                      a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->qpC[0], a->qpC[1], a->d_coefC[0], a->d_coefC[1],
-                                                      a->d_reconCTable, a->d_cu_sseC, a->d_cu_numsigC);
-        return launch_cu_chroma_residual<uint16_t>(c, fcb, fcr, a->d_refCbTable, a->d_refCrTable, a->cstride, a->d_cus, a->d_tus + tu0, ntu,
-                                                   a->d_cu_jobs, a->p.numRefs, a->d_me_out, a->qpC[0], a->qpC[1], a->d_coefC[0], a->d_coefC[1],
-                                                   a->d_reconCTable, a->d_cu_sseC, a->d_cu_numsigC);
-    }
+    if ((stages & 8) && ntu > 0 && an_residual(a, true, cu0, ncu, tu0, ntu)) return -1;
     return 0;
 }
 
@@ -315,7 +312,7 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     else if (p->subme < 0 || p->subme > 7) bad = "x265cu_analyser_create: subme outside 0..7";
     else if (p->width <= 0 || p->height <= 0 || (p->width & 7) || (p->height & 7))
         bad = "x265cu_analyser_create: width and height not positive multiples of 8";
-    // the quantiser's QPs: 0..51 + QP_BD_OFFSET (quant.cpp:224); k_cu_residual has scales for rem = qp % 6 in 0..5 only
+    // the quantiser's QPs: 0..51 + QP_BD_OFFSET (quant.cpp:224); resid_quant has scales for rem = qp % 6 in 0..5 only
     else if (p->qp < 0 || p->qp > 51 + 6 * (p->depth - 8))
         bad = "x265cu_analyser_create: qp outside 0..51 + 6 * (depth - 8)";
     else if (!isfinite(p->lambda) || p->lambda < 0)
@@ -518,7 +515,7 @@ int x265cu_analyser_load_chroma(x265cu_analyser* a, const void* cb_host, const v
     return 0;
 }
 
-// ---- 4:2:0 chroma residual chain (stage bit 3, chroma_resid.cuh) ----
+// ---- 4:2:0 chroma residual chain (stage bit 3, resid.cuh) ----
 int x265cu_analyser_enable_chroma_residual(x265cu_analyser* a, int cbQpOffset, int crQpOffset)
 {
     const char* bad = NULL;

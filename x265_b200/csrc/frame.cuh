@@ -1,11 +1,9 @@
 // x265_b200/csrc/frame.cuh -- frame-level fused kernels of the CTU-analysis pipeline (DESIGN.md):
 //   k_build_me_jobs : PU geometry table + predictor field -> motionEstimate jobs
 //                     (Search::setSearchRange search.cpp:2724-2768, CUData::clipMv cudata.cpp:1915-1928)
-//   k_cu_residual   : per TU, fully on-chip: best-ref select -> luma MC (predict.cpp:245-266) -> sub_ps
-//                     -> dct -> quant -> dequant_normal -> idct / DC shortcut -> add_ps -> sse_pp
-//                     (search.cpp:3178 estimateResidualQT; quant.cpp:397-470, :543-605 non-RDOQ path)
 //   k_intra_search  : per CU (8/16/32): neighbours from the source plane, 1:2:1 filter, 35 predictions
 //                     evaluated in registers, SA8D by an 8-lane shuffle Hadamard (search.cpp:1358-1444)
+// The residual chain of the luma and chroma planes (k_cu_residual) is in resid.cuh.
 #pragma once
 #include "common.cuh"
 #include "interp.cuh"
@@ -50,213 +48,6 @@ __global__ void k_pack_me(const int32_t* __restrict__ me_out, int n, int2* __res
     if (i >= n) return;
     int4 v = ((const int4*)me_out)[i];
     packed[i] = make_int2(v.x, (int)(((uint32_t)(uint16_t)(int16_t)v.y) | ((uint32_t)(uint16_t)(int16_t)v.z << 16)));
-}
-
-// ---------------------------------------------------------------------------------------------
-template <typename P>
-__global__ void __launch_bounds__(256) k_cu_residual(const P* __restrict__ fenc, const P* const* __restrict__ refs, int stride,
-                                                     const CuDesc* __restrict__ cus, const TuDesc* __restrict__ tus, int ntu,
-                                                     const int32_t* __restrict__ cu_jobs, int numRefs, const int32_t* __restrict__ me_out,
-                                                     int qp, int16_t* __restrict__ coef, P* const* __restrict__ recon,
-                                                     unsigned long long* __restrict__ cu_sse, uint32_t* __restrict__ cu_numsig, int32_t* __restrict__ cu_ref)
-{
-    constexpr int DEPTH = PixTraits<P>::depth;
-    constexpr int maxv = PixTraits<P>::maxv;
-    __shared__ int16_t s_win[39 * 40];     // (T+7)^2 source window
-    __shared__ int16_t s_mid[39 * 32];     // hps(rowExt) intermediate
-    __shared__ int16_t s_pred[32 * 32];
-    __shared__ int16_t s_a[32 * 34];       // rows padded to 34 in the forward passes (bank-conflict-free column reads)
-    __shared__ int16_t s_b[32 * 34];
-    __shared__ int8_t  s_m[32 * 32];
-    __shared__ int s_red[8];
-    __shared__ int s_lvl0;                 // quantised DC level of the TU
-    __shared__ unsigned long long s_red64[8];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-    for (int t = blockIdx.x; t < ntu; t += gridDim.x)
-    {
-        const TuDesc tu = tus[t];
-        const CuDesc cu = cus[tu.cu];
-        const int S = cu.size, T = S > 32 ? 32 : S, NN = T * T;
-        const int lg = 31 - __clz(T);
-        // best reference by ME cost, ties -> lowest index
-        int best = 0, bcost = 0x7fffffff;
-        for (int r = 0; r < numRefs; r++)
-        {
-            int c = me_out[(size_t)cu_jobs[tu.cu * numRefs + r] * 4];
-            if (c < bcost) { bcost = c; best = r; }
-        }
-        const int32_t* mo = me_out + (size_t)cu_jobs[tu.cu * numRefs + best] * 4;
-        const int qx = mo[1], qy = mo[2], xf = qx & 3, yf = qy & 3;
-        const int px = cu.x + tu.tx, py = cu.y + tu.ty;
-        const P* src = refs[best] + (size_t)py * stride + px + (qx >> 2) + (ptrdiff_t)(qy >> 2) * stride;
-        __syncthreads();
-        for (int i = tid; i < NN; i += blockDim.x) s_m[i] = d_dct[lg - 2][i];
-        // ---- luma MC into s_pred ----
-        if (!(xf | yf))
-        {
-            for (int i = tid; i < NN; i += blockDim.x) { int y = i >> lg, x = i & (T - 1); s_pred[i] = (int16_t)src[(ptrdiff_t)y * stride + x]; }
-        }
-        else
-        {
-            const int hl = xf ? 3 : 0, vt = yf ? 3 : 0;
-            const int ww = T + (xf ? 7 : 0), wh = T + (yf ? 7 : 0);
-            for (int i = tid; i < ww * wh; i += blockDim.x)
-            {
-                int r = i / ww, c = i - r * ww;
-                s_win[r * 40 + c] = (int16_t)src[(ptrdiff_t)(r - vt) * stride + (c - hl)];
-            }
-            __syncthreads();
-            const int16_t* cx = c_lumaFilter[xf];
-            const int16_t* cy = c_lumaFilter[yf];
-            if (!yf)
-            {
-                for (int i = tid; i < NN; i += blockDim.x)
-                {
-                    int y = i >> lg, x = i & (T - 1), sum = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) sum += (int)s_win[y * 40 + x + k] * cx[k];
-                    s_pred[i] = (int16_t)interp_finish<DEPTH>(sum, 0);
-                }
-            }
-            else if (!xf)
-            {
-                for (int i = tid; i < NN; i += blockDim.x)
-                {
-                    int y = i >> lg, x = i & (T - 1), sum = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) sum += (int)s_win[(y + k) * 40 + x] * cy[k];
-                    s_pred[i] = (int16_t)interp_finish<DEPTH>(sum, 0);
-                }
-            }
-            else
-            {
-                for (int i = tid; i < T * wh; i += blockDim.x)
-                {
-                    int r = i >> lg, x = i & (T - 1), sum = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) sum += (int)s_win[r * 40 + x + k] * cx[k];
-                    s_mid[r * 32 + x] = (int16_t)interp_finish<DEPTH>(sum, 1);
-                }
-                __syncthreads();
-                for (int i = tid; i < NN; i += blockDim.x)
-                {
-                    int y = i >> lg, x = i & (T - 1), sum = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) sum += (int)s_mid[(y + k) * 32 + x] * cy[k];
-                    s_pred[i] = (int16_t)interp_finish<DEPTH>(sum, 2);
-                }
-            }
-        }
-        __syncthreads();
-        // ---- residual ----
-        const P* fe = fenc + (size_t)py * stride + px;
-        for (int i = tid; i < NN; i += blockDim.x) { int y = i >> lg, x = i & (T - 1); s_a[y * 34 + x] = (int16_t)((int)fe[(size_t)y * stride + x] - (int)s_pred[i]); }
-        __syncthreads();
-        // ---- forward DCT: two passes (dct.cpp:83-240, 442-525) ----
-        {
-            const int sh1 = lg - 1 + (DEPTH - 8), sh2 = lg + 6;
-            for (int i = tid; i < NN; i += blockDim.x)
-            {
-                int k = i >> lg, jj = i & (T - 1), acc = 0;
-                for (int q = 0; q < T; q++) acc += (int)s_m[k * T + q] * s_a[jj * 34 + q];
-                s_b[k * 34 + jj] = (int16_t)((acc + (1 << (sh1 - 1))) >> sh1);
-            }
-            __syncthreads();
-            for (int i = tid; i < NN; i += blockDim.x)
-            {
-                int k = i >> lg, jj = i & (T - 1), acc = 0;
-                for (int q = 0; q < T; q++) acc += (int)s_m[k * T + q] * s_b[jj * 34 + q];
-                s_a[i] = (int16_t)((acc + (1 << (sh2 - 1))) >> sh2);           // coefficients back in linear k*T + j order
-            }
-            __syncthreads();
-        }
-        // ---- quant (dct.cpp:664-686; quant.cpp:411,465-466) + dequant (dct.cpp:612-634; quant.cpp:556,567) ----
-        const int per = qp / 6, rem = qp - per * 6;
-        const int quantScale = rem == 0 ? 26214 : rem == 1 ? 23302 : rem == 2 ? 20560 : rem == 3 ? 18396 : rem == 4 ? 16384 : 14564;
-        const int invScale = (rem == 0 ? 40 : rem == 1 ? 45 : rem == 2 ? 51 : rem == 3 ? 57 : rem == 4 ? 64 : 72) << per;
-        const int transformShift = 15 - DEPTH - lg;
-        const int qbits = 14 + per + transformShift;
-        const int add = 85 << (qbits - 9);
-        const int dqshift = 20 - 14 - transformShift;
-        int16_t* qout = coef + cu.coef_off + (size_t)((tu.ty / T) * (S / T) + (tu.tx / T)) * NN;
-        int cnt = 0;
-        for (int i = tid; i < NN; i += blockDim.x)
-        {
-            int c = s_a[i];
-            int tmp = abs(c) * quantScale;
-            int lvl = (tmp + add) >> qbits;
-            cnt += (lvl != 0);
-            if (c < 0) lvl = -lvl;
-            int q = clip16(lvl);
-            qout[i] = (int16_t)q;
-            if (i == 0) s_lvl0 = q;
-            s_b[i] = (int16_t)clip16((q * invScale + (1 << (dqshift - 1))) >> dqshift);      // dequantised
-        }
-        cnt = warp_sum(cnt);
-        if (lane == 0) s_red[warp] = cnt;
-        __syncthreads();
-        int numSig = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) numSig += s_red[w];
-        const int q0 = (int)s_b[0];        // dequantised DC (valid after the barrier)
-        // the reference tests coeff[0] != 0 on the QUANTISED level (quant.cpp:588)
-        const bool dcOnlyRef = (numSig == 1) && (s_lvl0 != 0);
-        __syncthreads();
-        // ---- inverse transform into s_a (residual') ----
-        if (numSig == 0)
-        {
-            for (int i = tid; i < NN; i += blockDim.x) s_a[i] = 0;
-        }
-        else if (dcOnlyRef)
-        {
-            const int shift_2nd = 12 - (DEPTH - 8) - 3;
-            const int dc = (((q0 + 1) >> 1) * 8 + (1 << (shift_2nd - 1))) >> shift_2nd;
-            for (int i = tid; i < NN; i += blockDim.x) s_a[i] = (int16_t)dc;
-        }
-        else
-        {
-            const int sh1 = 7, sh2 = 12 - (DEPTH - 8);
-            for (int i = tid; i < NN; i += blockDim.x)
-            {
-                int jj = i >> lg, i2 = i & (T - 1), acc = 0;
-                for (int q = 0; q < T; q++) acc += (int)s_m[q * T + i2] * s_b[q * T + jj];
-                s_a[i] = (int16_t)clip16((acc + (1 << (sh1 - 1))) >> sh1);
-            }
-            __syncthreads();
-            for (int i = tid; i < NN; i += blockDim.x)
-            {
-                int jj = i >> lg, i2 = i & (T - 1), acc = 0;
-                for (int q = 0; q < T; q++) acc += (int)s_m[q * T + i2] * s_a[q * T + jj];
-                s_b[i] = (int16_t)clip16((acc + (1 << (sh2 - 1))) >> sh2);
-            }
-            __syncthreads();
-            for (int i = tid; i < NN; i += blockDim.x) s_a[i] = s_b[i];
-        }
-        __syncthreads();
-        // ---- reconstruction + distortion ----
-        const int dIdx = S == 64 ? 0 : (S == 32 ? 1 : (S == 16 ? 2 : 3));
-        P* rc = recon[dIdx] + (size_t)py * stride + px;
-        unsigned long long sse = 0;
-        for (int i = tid; i < NN; i += blockDim.x)
-        {
-            int y = i >> lg, x = i & (T - 1);
-            int v = numSig ? clip3i(0, maxv, (int)s_pred[i] + (int)s_a[i]) : (int)s_pred[i];
-            rc[(size_t)y * stride + x] = (P)v;
-            int d = (int)fe[(size_t)y * stride + x] - v;
-            sse += (unsigned)(d * d);
-        }
-        sse = warp_sum64(sse);
-        if (lane == 0) s_red64[warp] = sse;
-        __syncthreads();
-        if (tid == 0)
-        {
-            unsigned long long tot = 0;
-            for (int w = 0; w < (int)(blockDim.x >> 5); w++) tot += s_red64[w];
-            atomicAdd(&cu_sse[tu.cu], tot);
-            atomicAdd(&cu_numsig[tu.cu], (uint32_t)numSig);
-            cu_ref[tu.cu] = best;
-        }
-    }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -54,24 +54,28 @@ static inline int geometry_cu_parts(int size, int rect, int amp, int part[13][4]
     return n;
 }
 
-// ---- 4:2:0 chroma residual stage (analyser stage bit 3) ----
+// ---- residual stages: TU placement per plane ----
 #ifdef __CUDACC__
 #define GEO_HD __host__ __device__ __forceinline__
 #else
 #define GEO_HD inline
 #endif
 
-// The chroma TU of a luma TU (T = min(S, 32)): (T/2) x (T/2) at half the luma coordinates.  Its levels start at
-// coef_off / 4 + (TU index in the CU) * (T/2)^2, so each chroma plane holds ncoef / 4 levels in the luma TU order.
-struct ChromaTu { int x, y, size; int64_t off; };
-GEO_HD ChromaTu geometry_chroma_tu(const CuDesc& cu, const TuDesc& tu)
+// The TU of a plane subsampled by `sub` (0 luma, 1 4:2:0 chroma) for a luma TU (T = min(S, 32)): (T >> sub) square at the
+// luma coordinates >> sub.  Its levels start at coef_off >> (2 * sub) + (TU index in the CU) * (T >> sub)^2, so a plane
+// holds ncoef >> (2 * sub) levels in the luma TU order.
+struct PlaneTu { int x, y, size; int64_t off; };
+GEO_HD PlaneTu geometry_plane_tu(const CuDesc& cu, const TuDesc& tu, int sub)
 {
-    const int S = cu.size, T = S > 32 ? 32 : S, Tc = T >> 1;
-    ChromaTu c;
-    c.x = (cu.x + tu.tx) >> 1; c.y = (cu.y + tu.ty) >> 1; c.size = Tc;
-    c.off = cu.coef_off / 4 + (int64_t)((tu.ty / T) * (S / T) + tu.tx / T) * Tc * Tc;
-    return c;
+    const int S = cu.size, T = S > 32 ? 32 : S, Tp = T >> sub;
+    PlaneTu p;
+    p.x = (cu.x + tu.tx) >> sub; p.y = (cu.y + tu.ty) >> sub; p.size = Tp;
+    p.off = (cu.coef_off >> (2 * sub)) + (int64_t)((tu.ty / T) * (S / T) + tu.tx / T) * Tp * Tp;
+    return p;
 }
+// the 4:2:0 chroma TU of a luma TU
+typedef PlaneTu ChromaTu;
+GEO_HD ChromaTu geometry_chroma_tu(const CuDesc& cu, const TuDesc& tu) { return geometry_plane_tu(cu, tu, 1); }
 
 // Quant::setChromaQP (quant.cpp:221-244) for 4:2:0: qp is the analyser's quantiser QP (QP_BD_OFFSET included), offset the
 // plane's PPS + slice offset (-12..12).  Returns the plane's quantiser QP.

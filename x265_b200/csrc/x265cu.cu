@@ -10,7 +10,7 @@
 #include "me.cuh"
 #include "predcost.cuh"
 #include "frame.cuh"
-#include "chroma_resid.cuh"
+#include "resid.cuh"
 #include "lookahead.cuh"
 #include <math.h>
 #include <mutex>
