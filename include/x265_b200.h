@@ -294,6 +294,42 @@ int x265cu_analyser_fetch_chroma(x265cu_analyser*, int what, void* host); /* 0 /
 void* x265cu_analyser_recon_plane_chroma(x265cu_analyser*, int depthIdx, int plane, int* cstride);
 int x265cu_analyser_recon_to_ref_chroma(x265cu_analyser*, int depthIdx, int refIdx, int ctuRow0, int ctuRow1);
 int x265cu_analyser_ref_chroma_updated(x265cu_analyser*, int idx);     /* re-extend the chroma borders of ref idx */
+/* device address of chroma plane `plane` (0 Cb, 1 Cr) of ref idx at pixel (0,0) and its stride in elements (NULL before
+ * enable_chroma()); the chroma twin of x265cu_analyser_ref_plane */
+void* x265cu_analyser_ref_plane_chroma(x265cu_analyser*, int idx, int plane, int* cstride);
+
+/* ---------- frame-level deblocking (common/deblock.cpp) ----------
+ * The host's final decisions, one record per 4x4 luma unit in raster order over the picture (width / 4 records per row),
+ * mirroring the CUData fields Deblock reads. */
+typedef struct {
+    int8_t  qp;             /* CUData::m_qp (spec QP, -QpBdOffset..51) */
+    uint8_t flags;          /* bit 0 intra (isIntra), bit 1 luma cbf of the unit's TU (getCbf(.., TEXT_LUMA, tuDepth)),
+                               bit 2 cu_transquant_bypass (m_tqBypass) */
+    uint8_t log2CuSize;     /* 3..6 */
+    uint8_t partSize;       /* PartSize: SIZE_2Nx2N 0 .. SIZE_nRx2N 7 */
+    uint8_t tuDepth;        /* m_tuDepth */
+    int8_t  refPic[2];      /* identity of the L0 / L1 reference PICTURE, -1 = list unused.  Deblock compares Frame pointers,
+                               not indices (deblock.cpp:210-225): equal ids = the same picture, in either list */
+    int16_t mv[2][2];       /* quarter-pel m_mv[list] */
+} x265cu_deblock_unit;      /* 16 bytes */
+
+typedef struct {
+    int32_t sliceType;                      /* B_SLICE 0, P_SLICE 1, I_SLICE 2 (slice.h) */
+    int32_t betaOffsetDiv2, tcOffsetDiv2;   /* PPS, -6..6 */
+    int32_t cbQpOffset, crQpOffset;         /* PPS chromaQpOffset[2], -12..12 (the slice offsets do not enter deblocking) */
+    int32_t transquantBypass;               /* PPS bTransquantBypassEnabled, 0 or 1 */
+} x265cu_deblock_params;
+
+/* Deblocks one picture (a single slice: only picture borders are unfiltered edges) in place on the context's stream, as
+ * Deblock::deblockCTU over every CTU in FrameFilter's order does (framefilter.cpp:457-516): every vertical edge, then every
+ * horizontal edge of the result; luma edges on the 8x8 grid, 4:2:0 chroma edges every 8 chroma samples.  Planes point at
+ * pixel (0,0), strides in elements; cb_dev == cr_dev == NULL filters luma only (4:0:0).  units_dev: (width / 4) x
+ * (height / 4) records.  Returns -1 with x265cu_last_error(), before any launch, for depth not 8 or 10, width or height not a
+ * positive multiple of 8, a stride smaller than the row, parameters outside the ranges above, a NULL luma or unit pointer,
+ * or only one NULL chroma pointer.  Any byte values in the map are read safely: a unit outside the documented ranges gives
+ * unspecified pixels, never a fault. */
+int x265cu_deblock_frame(x265cu_ctx*, int depth, void* luma_dev, int stride, void* cb_dev, void* cr_dev, int cstride,
+                         int width, int height, const x265cu_deblock_unit* units_dev, const x265cu_deblock_params* params);
 
 /* ---------- lookahead frame costs (BASELINE configs[1]; slicetype.cpp:696-805, 3115-3388) ----------
  * All pointers are device pointers.  Planes are the 4 lowres hpel planes of a frame (origin pixel,

@@ -633,6 +633,14 @@ int x265cu_analyser_ref_chroma_updated(x265cu_analyser* a, int idx)
     return 0;
 }
 
+// device address of chroma plane `plane` of reference idx at its origin pixel, and the chroma stride in elements
+void* x265cu_analyser_ref_plane_chroma(x265cu_analyser* a, int idx, int plane, int* cstride)
+{
+    if (!a->chromaOn || idx < 0 || idx >= a->p.numRefs || plane < 0 || plane > 1) return NULL;
+    *cstride = a->cstride;
+    return a->d_refC[idx][plane] + a->cOrgBytes;
+}
+
 int x265cu_analyser_run_resident(x265cu_analyser* a, int stages) { return an_run(a, stages, 0, a->ctuRows); }
 
 // ---- CTU-row shards (the WPP row partition of SURVEY 8(e): frameencoder.cpp:850-868 enables row r once the

@@ -6,6 +6,8 @@
 // so all kernels read an unmodified input block and write a separate output block: one thread per sample, rows that pass
 // signs to the next row (E1 / E2 / E3 and the statistics) synchronise once per row.
 // Blocks are staged compactly by the per-call thunks (thunks.cuh); each kernel documents its layout.
+// The frame-level deblocking (k_deblock_frame, x265cu_deblock_frame) is the exception: it filters whole planes in place, since
+// the edges of one direction touch disjoint samples (see there).
 #pragma once
 #include "common.cuh"
 
@@ -96,7 +98,46 @@ __global__ void k_sao_b0(const P* __restrict__ in, P* __restrict__ out, const in
     }
 }
 
-// pelFilterLumaStrong_c (:140-160) / pelFilterChroma_c (:167-181).  in / out: 4 lines x 8 samples m0..m7 (m4 = src[0]).
+// ---- deblocking, one line across an edge: m[0..7] = the samples p3 p2 p1 p0 | q0 q1 q2 q3 (m[4] = src[0] of the reference),
+// read as int16_t of the pixel as the reference does.  Each helper replaces the samples its filter writes.
+
+// pelFilterLumaStrong_c (loopfilter.cpp:140-160): m[1..6], no pixel clip (the tc bounds keep them in range)
+__device__ __forceinline__ void luma_strong_line(int* m, int tcP, int tcQ)
+{
+    const int m0 = m[0], m1 = m[1], m2 = m[2], m3 = m[3], m4 = m[4], m5 = m[5], m6 = m[6], m7 = m[7];
+    m[1] = clip3i(-tcP, tcP, ((2 * m0 + 3 * m1 + m2 + m3 + m4 + 4) >> 3) - m1) + m1;
+    m[2] = clip3i(-tcP, tcP, ((m1 + m2 + m3 + m4 + 2) >> 2) - m2) + m2;
+    m[3] = clip3i(-tcP, tcP, ((m1 + 2 * m2 + 2 * m3 + 2 * m4 + m5 + 4) >> 3) - m3) + m3;
+    m[4] = clip3i(-tcQ, tcQ, ((m2 + 2 * m3 + 2 * m4 + 2 * m5 + m6 + 4) >> 3) - m4) + m4;
+    m[5] = clip3i(-tcQ, tcQ, ((m3 + m4 + m5 + m6 + 2) >> 2) - m5) + m5;
+    m[6] = clip3i(-tcQ, tcQ, ((m3 + m4 + m5 + 3 * m6 + 2 * m7 + 4) >> 3) - m6) + m6;
+}
+
+// pelFilterLuma (deblock.cpp:278-315), the normal filter: m[2..5].  maskP1 / maskQ1 already include maskP / maskQ.
+template <typename P>
+__device__ __forceinline__ void luma_normal_line(int* m, int tc, int maskP, int maskQ, int maskP1, int maskQ1)
+{
+    const int m1 = m[1], m2 = m[2], m3 = m[3], m4 = m[4], m5 = m[5], m6 = m[6];
+    int delta = (9 * (m4 - m3) - 3 * (m5 - m2) + 8) >> 4;
+    if (abs(delta) >= tc * 10) return;
+    delta = clip3i(-tc, tc, delta);
+    const int tc2 = tc >> 1;
+    m[3] = clipP<P>(m3 + (delta & maskP));
+    m[4] = clipP<P>(m4 - (delta & maskQ));
+    if (maskP1) m[2] = clipP<P>(m2 + clip3i(-tc2, tc2, (((m1 + m3 + 1) >> 1) - m2 + delta) >> 1));
+    if (maskQ1) m[5] = clipP<P>(m5 + clip3i(-tc2, tc2, (((m6 + m4 + 1) >> 1) - m5 - delta) >> 1));
+}
+
+// pelFilterChroma_c (loopfilter.cpp:167-181): m[3], m[4] from m[2..5]
+template <typename P>
+__device__ __forceinline__ void chroma_line(int* m, int tc, int maskP, int maskQ)
+{
+    const int delta = clip3i(-tc, tc, ((((m[4] - m[3]) * 4) + m[2] - m[5] + 4) >> 3));
+    m[3] = clipP<P>(m[3] + (delta & maskP));
+    m[4] = clipP<P>(m[4] - (delta & maskQ));
+}
+
+// Per-call table entries pelFilterLumaStrong / pelFilterChroma.  in / out: 4 lines x 8 samples m0..m7 (m4 = src[0]).
 template <typename P>
 __global__ void k_deblock_luma_strong(const P* __restrict__ in, P* __restrict__ out, int tcP, int tcQ)
 {
@@ -105,27 +146,206 @@ __global__ void k_deblock_luma_strong(const P* __restrict__ in, P* __restrict__ 
     int m[8];
 #pragma unroll
     for (int k = 0; k < 8; k++) m[k] = (int)(int16_t)in[i * 8 + k];
-    P* o = out + i * 8;
+    luma_strong_line(m, tcP, tcQ);
 #pragma unroll
-    for (int k = 0; k < 8; k++) o[k] = (P)m[k];
-    o[1] = (P)(clip3i(-tcP, tcP, ((2 * m[0] + 3 * m[1] + m[2] + m[3] + m[4] + 4) >> 3) - m[1]) + m[1]);
-    o[2] = (P)(clip3i(-tcP, tcP, ((m[1] + m[2] + m[3] + m[4] + 2) >> 2) - m[2]) + m[2]);
-    o[3] = (P)(clip3i(-tcP, tcP, ((m[1] + 2 * m[2] + 2 * m[3] + 2 * m[4] + m[5] + 4) >> 3) - m[3]) + m[3]);
-    o[4] = (P)(clip3i(-tcQ, tcQ, ((m[2] + 2 * m[3] + 2 * m[4] + 2 * m[5] + m[6] + 4) >> 3) - m[4]) + m[4]);
-    o[5] = (P)(clip3i(-tcQ, tcQ, ((m[3] + m[4] + m[5] + m[6] + 2) >> 2) - m[5]) + m[5]);
-    o[6] = (P)(clip3i(-tcQ, tcQ, ((m[3] + m[4] + m[5] + 3 * m[6] + 2 * m[7] + 4) >> 3) - m[6]) + m[6]);
+    for (int k = 0; k < 8; k++) out[i * 8 + k] = (P)m[k];
 }
 template <typename P>
 __global__ void k_deblock_chroma(const P* __restrict__ in, P* __restrict__ out, int tc, int maskP, int maskQ)
 {
     const int i = threadIdx.x;
     if (i >= 4) return;
-    const int m2 = (int)(int16_t)in[i * 8 + 2], m3 = (int)(int16_t)in[i * 8 + 3], m4 = (int)(int16_t)in[i * 8 + 4], m5 = (int)(int16_t)in[i * 8 + 5];
-    const int delta = clip3i(-tc, tc, ((((m4 - m3) * 4) + m2 - m5 + 4) >> 3));
+    int m[8];
 #pragma unroll
-    for (int k = 0; k < 8; k++) out[i * 8 + k] = in[i * 8 + k];
-    out[i * 8 + 3] = (P)clipP<P>(m3 + (delta & maskP));
-    out[i * 8 + 4] = (P)clipP<P>(m4 - (delta & maskQ));
+    for (int k = 0; k < 8; k++) m[k] = (int)(int16_t)in[i * 8 + k];
+    chroma_line<P>(m, tc, maskP, maskQ);
+#pragma unroll
+    for (int k = 0; k < 8; k++) out[i * 8 + k] = (P)m[k];
+}
+
+// ---- frame-level deblocking (deblock.cpp, driven by the per-4x4 decision map of x265cu_deblock_frame) ----
+// Deblock::s_tcTable / s_betaTable (deblock.cpp:499-509) and g_chromaScale (constants.cpp:346), in global memory: the frame
+// kernels index them per lane.
+__device__ const uint8_t d_tcTable[54] = {
+    0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2,
+    2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 5, 5, 6, 6, 7, 8, 9, 10, 11, 13, 14, 16, 18, 20, 22, 24 };
+__device__ const uint8_t d_betaTable[52] = {
+    0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17,
+    18, 20, 22, 24, 26, 28, 30, 32, 34, 36, 38, 40, 42, 44, 46, 48, 50, 52, 54, 56, 58, 60, 62, 64 };
+__device__ const uint8_t d_chromaScale[70] = {
+    0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 29, 30, 31,
+    32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37, 38, 39, 40, 41, 42, 43, 44, 45, 46, 47, 48, 49, 50, 51,
+    51, 51, 51, 51, 51, 51, 51, 51, 51, 51, 51, 51 };
+
+struct DeblockArgs
+{
+    void* plane[3];                 // luma, Cb, Cr at pixel (0,0); plane[1] == NULL: luma only
+    int stride, cstride, width, height;
+    const x265cu_deblock_unit* units;
+    int sliceType, betaOffset, tcOffset, cbQpOffset, crQpOffset, bypass;   // offsets already doubled (deblock.cpp:328-329)
+};
+
+// Edge flag of the 8-sample edge at `pos` (x for vertical edges, y for horizontal ones) as Deblock::deblockCU leaves it at the Q
+// unit (deblock.cpp:90-93): the CU edge 2 (never the picture border: pos > 0 here), else a TU edge 2 (setEdgefilterTU), else an
+// internal PU edge 1 (setEdgefilterPU), else 0.
+template <int DIR>
+__device__ __forceinline__ int edge_flag(const x265cu_deblock_unit& q, int pos)
+{
+    const int log2S = min(max((int)q.log2CuSize, 3), 6), S = 1 << log2S;
+    const int o = pos & (S - 1);
+    if (o == 0) return 2;
+    const int T = S >> min((int)q.tuDepth, 3);
+    if ((o & (T - 1)) == 0) return 2;
+    const int ps = q.partSize, h = S >> 1, qu = S >> 2;
+    bool pu;
+    if (DIR == 0) pu = ((ps == 2 || ps == 3) && o == h) || (ps == 6 && o == qu) || (ps == 7 && o == S - qu);
+    else          pu = ((ps == 1 || ps == 3) && o == h) || (ps == 4 && o == qu) || (ps == 5 && o == S - qu);
+    return pu ? 1 : 0;
+}
+
+__device__ __forceinline__ bool mv_far(int ax, int ay, int bx, int by) { return abs(ax - bx) >= 4 || abs(ay - by) >= 4; }
+
+// Deblock::getBoundaryStrength (deblock.cpp:191-247) for an edge with flag != 0.  refPic ids stand for the Frame pointers the
+// reference compares; an id < 0 is an unused list (NULL, zero vector).
+__device__ __forceinline__ int boundary_strength(const x265cu_deblock_unit& p, const x265cu_deblock_unit& q, int flag, int sliceType)
+{
+    if ((p.flags | q.flags) & 1) return 2;
+    if (flag > 1 && ((p.flags | q.flags) & 2)) return 1;
+    const int rP0 = p.refPic[0] < 0 ? -1 : p.refPic[0], rQ0 = q.refPic[0] < 0 ? -1 : q.refPic[0];
+    const int rP1 = p.refPic[1] < 0 ? -1 : p.refPic[1], rQ1 = q.refPic[1] < 0 ? -1 : q.refPic[1];
+    const int p0x = rP0 >= 0 ? p.mv[0][0] : 0, p0y = rP0 >= 0 ? p.mv[0][1] : 0, q0x = rQ0 >= 0 ? q.mv[0][0] : 0, q0y = rQ0 >= 0 ? q.mv[0][1] : 0;
+    if (sliceType == 1) return (rP0 != rQ0 || mv_far(q0x, q0y, p0x, p0y)) ? 1 : 0;
+    const int p1x = rP1 >= 0 ? p.mv[1][0] : 0, p1y = rP1 >= 0 ? p.mv[1][1] : 0, q1x = rQ1 >= 0 ? q.mv[1][0] : 0, q1y = rQ1 >= 0 ? q.mv[1][1] : 0;
+    if ((rP0 == rQ0 && rP1 == rQ1) || (rP0 == rQ1 && rP1 == rQ0))
+    {
+        if (rP0 != rP1)
+        {
+            if (rP0 == rQ0) return (mv_far(q0x, q0y, p0x, p0y) || mv_far(q1x, q1y, p1x, p1y)) ? 1 : 0;
+            return (mv_far(q1x, q1y, p0x, p0y) || mv_far(q0x, q0y, p1x, p1y)) ? 1 : 0;
+        }
+        return ((mv_far(q0x, q0y, p0x, p0y) || mv_far(q1x, q1y, p1x, p1y)) && (mv_far(q1x, q1y, p0x, p0y) || mv_far(q0x, q0y, p1x, p1y))) ? 1 : 0;
+    }
+    return 1;
+}
+
+// One 4-line segment of every 8-sample edge of one direction, one thread each, in place (the filters of neighbouring edges
+// touch disjoint samples: reads 4 / writes 3 per side, 2 / 1 for chroma).  DIR 0 (EDGE_VER): x = edge index e (luma x = 8e,
+// e >= 1), y = unit row a.  DIR 1 (EDGE_HOR): x = unit column a, y = edge index e (luma y = 8e).  The thread of an even e and
+// an even a also filters the chroma segment of that edge (4:2:0: chroma edges every 8 chroma samples, 4 chroma lines = the
+// 8 luma lines from unit a; deblock.cpp:104-113, 456-460).
+template <typename P, int DIR>
+__global__ void __launch_bounds__(256) k_deblock_frame(const DeblockArgs a)
+{
+    const int gx = blockIdx.x * blockDim.x + threadIdx.x, gy = blockIdx.y * blockDim.y + threadIdx.y;
+    const int e = (DIR == 0 ? gx : gy) + 1, s = DIR == 0 ? gy : gx;
+    if (DIR == 0 ? (e >= (a.width >> 3) || s >= (a.height >> 2)) : (e >= (a.height >> 3) || s >= (a.width >> 2))) return;
+    const int upr = a.width >> 2;
+    const size_t iq = DIR == 0 ? (size_t)s * upr + 2 * e : (size_t)(2 * e) * upr + s;
+    const size_t ip = DIR == 0 ? iq - 1 : iq - upr;
+    const x265cu_deblock_unit uq = a.units[iq], up = a.units[ip];
+    const int flag = edge_flag<DIR>(uq, 8 * e);
+    if (!flag) return;
+    const int bs = boundary_strength(up, uq, flag, a.sliceType);
+    if (!bs) return;
+    int maskP = -1, maskQ = -1;
+    if (a.bypass)
+    {   // deblock.cpp:358-365, 469-476
+        maskP = (up.flags & 4) ? 0 : -1; maskQ = (uq.flags & 4) ? 0 : -1;
+        if (!(maskP | maskQ)) return;
+    }
+    constexpr int shift = PixTraits<P>::depth - 8;
+    const int qpA = ((int)up.qp + (int)uq.qp + 1) >> 1;
+
+    // luma (edgeFilterLuma, deblock.cpp:317-415)
+    {
+        P* src = (P*)a.plane[0];
+        const ptrdiff_t across = DIR == 0 ? 1 : a.stride, along = DIR == 0 ? a.stride : 1;
+        src += DIR == 0 ? (ptrdiff_t)(4 * s) * a.stride + 8 * e : (ptrdiff_t)(8 * e) * a.stride + 4 * s;
+        int m[4][8];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+#pragma unroll
+            for (int k = 0; k < 8; k++) m[i][k] = (int)(int16_t)src[i * along + (k - 4) * across];
+        const int beta = d_betaTable[clip3i(0, 51, qpA + a.betaOffset)] << shift;
+        const int dp0 = abs(m[0][1] - 2 * m[0][2] + m[0][3]), dq0 = abs(m[0][4] - 2 * m[0][5] + m[0][6]);
+        const int dp3 = abs(m[3][1] - 2 * m[3][2] + m[3][3]), dq3 = abs(m[3][4] - 2 * m[3][5] + m[3][6]);
+        const int d0 = dp0 + dq0, d3 = dp3 + dq3;
+        if (d0 + d3 < beta)
+        {
+            const int tc = d_tcTable[clip3i(0, 53, qpA + 2 * (bs - 1) + a.tcOffset)] << shift;
+            const int sb = beta >> 3, st = (tc * 5 + 1) >> 1;
+            const bool sw = 2 * d0 < (beta >> 2) && 2 * d3 < (beta >> 2) &&
+                            abs(m[0][0] - m[0][3]) + abs(m[0][7] - m[0][4]) < sb && abs(m[0][3] - m[0][4]) < st &&
+                            abs(m[3][0] - m[3][3]) + abs(m[3][7] - m[3][4]) < sb && abs(m[3][3] - m[3][4]) < st;
+            if (sw)
+            {
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+                {
+                    luma_strong_line(m[i], (2 * tc) & maskP, (2 * tc) & maskQ);
+#pragma unroll
+                    for (int k = 1; k < 7; k++) src[i * along + (k - 4) * across] = (P)m[i][k];
+                }
+            }
+            else
+            {
+                const int side = (beta + (beta >> 1)) >> 3;
+                const int maskP1 = (dp0 + dp3 < side ? -1 : 0) & maskP, maskQ1 = (dq0 + dq3 < side ? -1 : 0) & maskQ;
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+                {
+                    luma_normal_line<P>(m[i], tc, maskP, maskQ, maskP1, maskQ1);
+#pragma unroll
+                    for (int k = 2; k < 6; k++) src[i * along + (k - 4) * across] = (P)m[i][k];
+                }
+            }
+        }
+    }
+
+    // chroma (edgeFilterChroma, deblock.cpp:417-497): bs 2 only, the BS and QPs of the segment's first luma unit
+    if (a.plane[1] && bs == 2 && !(e & 1) && !(s & 1))
+    {
+        const ptrdiff_t across = DIR == 0 ? 1 : a.cstride, along = DIR == 0 ? a.cstride : 1;
+        const ptrdiff_t org = DIR == 0 ? (ptrdiff_t)(2 * s) * a.cstride + 4 * e : (ptrdiff_t)(4 * e) * a.cstride + 2 * s;
+#pragma unroll
+        for (int c = 0; c < 2; c++)
+        {
+            int qp = qpA + (c ? a.crQpOffset : a.cbQpOffset);
+            if (qp >= 30) qp = d_chromaScale[min(qp, 69)];
+            const int tc = d_tcTable[clip3i(0, 53, qp + 2 + a.tcOffset)] << shift;
+            P* src = (P*)a.plane[1 + c] + org;
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+            {
+                int m[8];
+#pragma unroll
+                for (int k = 2; k < 6; k++) m[k] = (int)(int16_t)src[i * along + (k - 4) * across];
+                chroma_line<P>(m, tc, maskP, maskQ);
+                src[i * along - across] = (P)m[3];
+                src[i * along] = (P)m[4];
+            }
+        }
+    }
+}
+
+// the two passes of x265cu_deblock_frame (arguments validated by the caller)
+template <typename P>
+static int launch_deblock_frame(x265cu_ctx* c, const DeblockArgs& a)
+{
+    const dim3 block(32, 8);
+    const int ne = (a.width >> 3) - 1, ns = a.height >> 2;             // vertical: edges x segments
+    if (ne > 0)
+    {
+        k_deblock_frame<P, 0><<<dim3((ne + 31) / 32, (ns + 7) / 8), block, 0, c->stream>>>(a);
+        CU_LAUNCH_CHECK(c);
+    }
+    const int nh = (a.height >> 3) - 1, nc = a.width >> 2;             // horizontal: segments x edges
+    if (nh > 0)
+    {
+        k_deblock_frame<P, 1><<<dim3((nc + 31) / 32, (nh + 7) / 8), block, 0, c->stream>>>(a);
+        CU_LAUNCH_CHECK(c);
+    }
+    return 0;
 }
 
 // ---- SAO statistics (sao.cpp:1762-1927).  stats / count: in/out (32 classes for BO, 5 for the edge types through s_eoTable).

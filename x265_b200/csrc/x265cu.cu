@@ -401,3 +401,31 @@ int x265cu_propagate_cost_batch(x265cu_ctx* c, int* dst, const uint16_t* propaga
 #include "analyser.cuh"
 #include "thunks.cuh"
 #include "la_weights.cuh"
+
+static_assert(sizeof(x265cu_deblock_unit) == 16 && sizeof(x265cu_deblock_params) == 24, "deblocking records (include/x265_b200.h)");
+
+extern "C" int x265cu_deblock_frame(x265cu_ctx* c, int depth, void* luma, int stride, void* cb, void* cr, int cstride,
+                                    int width, int height, const x265cu_deblock_unit* units, const x265cu_deblock_params* p)
+{
+    cudaSetDevice(c->device);
+    const bool chroma = cb || cr;
+    const char* bad = NULL;
+    if (depth != 8 && depth != 10) bad = "x265cu_deblock_frame: depth must be 8 or 10";
+    else if (width <= 0 || height <= 0 || (width & 7) || (height & 7)) bad = "x265cu_deblock_frame: width and height must be positive multiples of 8";
+    else if (!luma || !units || !p) bad = "x265cu_deblock_frame: NULL luma plane, unit map or parameters";
+    else if (chroma && (!cb || !cr)) bad = "x265cu_deblock_frame: give both chroma planes or neither";
+    else if (stride < width || (chroma && cstride < width / 2)) bad = "x265cu_deblock_frame: stride smaller than the row";
+    else if (p->sliceType < 0 || p->sliceType > 2) bad = "x265cu_deblock_frame: sliceType must be 0 (B), 1 (P) or 2 (I)";
+    else if (p->betaOffsetDiv2 < -6 || p->betaOffsetDiv2 > 6 || p->tcOffsetDiv2 < -6 || p->tcOffsetDiv2 > 6)
+        bad = "x265cu_deblock_frame: beta / tc offsets (div 2) must be in -6..6";
+    else if (p->cbQpOffset < -12 || p->cbQpOffset > 12 || p->crQpOffset < -12 || p->crQpOffset > 12)
+        bad = "x265cu_deblock_frame: chroma QP offsets must be in -12..12";
+    else if (p->transquantBypass != 0 && p->transquantBypass != 1) bad = "x265cu_deblock_frame: transquantBypass must be 0 or 1";
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    lf::DeblockArgs a;
+    a.plane[0] = luma; a.plane[1] = chroma ? cb : NULL; a.plane[2] = chroma ? cr : NULL;
+    a.stride = stride; a.cstride = cstride; a.width = width; a.height = height; a.units = units;
+    a.sliceType = p->sliceType; a.betaOffset = p->betaOffsetDiv2 * 2; a.tcOffset = p->tcOffsetDiv2 * 2;
+    a.cbQpOffset = p->cbQpOffset; a.crQpOffset = p->crQpOffset; a.bypass = p->transquantBypass;
+    return depth == 8 ? lf::launch_deblock_frame<uint8_t>(c, a) : lf::launch_deblock_frame<uint16_t>(c, a);
+}

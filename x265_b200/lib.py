@@ -37,6 +37,17 @@ PRED_SAD, PRED_SATD, PRED_CHROMA, PRED_AVG_PP = 0, 1, 1, 2
 ME_JOB = np.dtype([("offset", "<i4"), ("ref", "<i2"), ("pw", "i1"), ("ph", "i1"), ("mvmin", "<i2", 2), ("mvmax", "<i2", 2),
                    ("qmvp", "<i2", 2), ("mvc", "<i2", 8), ("numCand", "i1"), ("method", "i1"), ("subme", "i1"), ("merange", "i1")], align=True)
 assert CMP_JOB.itemsize == 32 and BLK_JOB.itemsize == 56 and INTERP_JOB.itemsize == 32 and ME_JOB.itemsize == 40
+# x265cu_deblock_unit: one record per 4x4 luma unit, raster order; flags bit 0 intra, bit 1 luma cbf, bit 2 tq-bypass
+DEBLOCK_UNIT = np.dtype([("qp", "i1"), ("flags", "u1"), ("log2CuSize", "u1"), ("partSize", "u1"), ("tuDepth", "u1"),
+                         ("refPic", "i1", 2), ("mv", "<i2", (2, 2))], align=True)
+assert DEBLOCK_UNIT.itemsize == 16
+B_SLICE, P_SLICE, I_SLICE = 0, 1, 2
+
+
+class DeblockParams(C.Structure):
+    """x265cu_deblock_params (include/x265_b200.h)"""
+    _fields_ = [("sliceType", C.c_int32), ("betaOffsetDiv2", C.c_int32), ("tcOffsetDiv2", C.c_int32), ("cbQpOffset", C.c_int32),
+                ("crQpOffset", C.c_int32), ("transquantBypass", C.c_int32)]
 
 OPS_CMP = dict(sad=0, satd=1, sa8d=2, sse_pp=3, sse_ss=4, ssd_s=5, var=6, psy=7)
 OPS_BLK = dict(copy_pp=0, copy_ss=1, copy_sp=2, copy_ps=3, sub_ps=4, add_ps=5, pixelavg_pp=6, addAvg=7, p2s=8, transpose=9,
@@ -86,6 +97,7 @@ _PROTOS = {
     "x265cu_me_batch": (I, [P, I, P, I, P, I, I, P, I, P, I, P]),
     "x265cu_me_batch_chroma": (I, [P, I, P, I, P, I, P, P, I, P, I, P]),
     "x265cu_pred_cost_batch": (I, [P, I, P, I, P, I, P, P, I, P]),
+    "x265cu_deblock_frame": (I, [P, I, P, I, P, P, I, I, I, P, P]),
 }
 
 
@@ -232,6 +244,13 @@ class Lib:
                                                            padoffset, intra.ctypes.data, st.ctypes.data, wp.ctypes.data))
         return tuple(int(x) for x in wp)
 
+    def deblock_frame(self, depth, luma, stride, cb, cr, cstride, width, height, units, params):
+        """x265cu_deblock_frame: deblocks a picture in place on the context's stream.  luma / cb / cr: device addresses (ints)
+        of pixel (0,0), cb = cr = None for luma only; units: device buffer (or address) of (width / 4) x (height / 4)
+        DEBLOCK_UNIT records; params: DeblockParams."""
+        uptr = units.ptr if isinstance(units, DeviceBuffer) else units
+        self.check(self.L.x265cu_deblock_frame(self.ctx, depth, luma, stride, cb, cr, cstride, width, height, uptr, C.byref(params)))
+
     def mvcost_table(self, lam, rng):
         t = np.zeros(2 * rng + 1, np.uint16)
         self.L.x265cu_mvcost_table(C.c_double(lam), rng, t.ctypes.data)
@@ -294,6 +313,7 @@ _AN_PROTOS = {
     "x265cu_analyser_recon_plane_chroma": (P, [P, I, I, C.POINTER(I)]),
     "x265cu_analyser_recon_to_ref_chroma": (I, [P, I, I, I, I]),
     "x265cu_analyser_ref_chroma_updated": (I, [P, I]),
+    "x265cu_analyser_ref_plane_chroma": (P, [P, I, I, C.POINTER(I)]),
 }
 STAGE_CHROMA_RESIDUAL = 8                 # analyser stage bit 3 (x265cu_analyser_enable_chroma_residual)
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
@@ -450,6 +470,14 @@ class Analyser:
 
     def ref_chroma_updated(self, idx):
         self.lib.check(self.lib.L.x265cu_analyser_ref_chroma_updated(self.h, idx))
+
+    def ref_plane_chroma(self, idx, plane):
+        """(device address of pixel (0,0), stride in elements) of chroma plane `plane` (0 Cb, 1 Cr) of reference idx."""
+        st = I()
+        p = self.lib.L.x265cu_analyser_ref_plane_chroma(self.h, idx, plane, C.byref(st))
+        if not p:
+            raise RuntimeError("x265cu_analyser_ref_plane_chroma(%d, %d): no such plane (enable_chroma() first)" % (idx, plane))
+        return p, st.value
 
     def h2d_bytes(self, field):
         return self.width * self.height * np.dtype(self.dtype).itemsize + field.nbytes
