@@ -1,5 +1,6 @@
 """Kernel times of the sub-pel phase of the frame analyser: the phase-plane build (k_interp_rows over plane tiles) and the
-sub-pel launches (the cells' k_me_subpel_cell, or k_me<P, 3, 0, ...> without it, and k_me<P, 3, 1, ...>), from torch.profiler, at bench.py's c3 and c4 shapes.  Reports the build's
+sub-pel launches (the groups' k_me_subpel_group and k_me_subpel_cell, or k_me<P, 3, 0, ...> without them, and k_me<P, 3, 1, ...>
+for what is left), from torch.profiler, at bench.py's c3 and c4 shapes.  Reports the build's
 achieved bandwidth against the H100 SXM data-sheet HBM3 figure (3.35 TB/s), counting one plane read and 15 planes
 written per reference over the built rectangle (analyser.cuh: AN_PLANE_X / AN_PLANE_Y), with the card's name and power
 limit.  Needs a GPU; prints one JSON line per config.
@@ -46,7 +47,7 @@ def kernel_ms(prof, steps):
         if "k_interp_rows" in n:
             build += t
             names[n] = t / 1000.0 / steps
-        elif (n.startswith("void k_me<") and ", 3, " in n) or "k_me_subpel_cell" in n:
+        elif (n.startswith("void k_me<") and ", 3, " in n) or "k_me_subpel_" in n:
             subpel[n] = t / 1000.0 / steps
     return build / 1000.0 / steps, subpel, names
 

@@ -693,6 +693,16 @@ __device__ __noinline__ int me_subpel_compare_planes(const MeCtx<P>& c, int qx, 
 template <typename P>
 __device__ __forceinline__ int me_subpel_class(const MeCtx<P>& c) { return (c.pow2 && c.w <= 16 && c.h <= 16) ? 0 : 1; }
 
+// Which kernel refines a PU of the frame analyser's job groups at sub-pel (me_window.cuh): 0 = k_me_subpel_cell (class 0),
+// 1 = k_me_subpel_group (the 2Nx2N / 2NxN / Nx2N PUs of the CUs 32 and 64: power-of-two sides of 16 to 64, at most 2:1),
+// 2 = the per-PU class-1 launch (AMP parts with a 12 / 24 / 48 side or a 4:1 shape of a CU 32 / CU 64)
+__host__ __device__ __forceinline__ int me_subpel_kernel(int pw, int ph)
+{
+    if ((pw & (pw - 1)) | (ph & (ph - 1))) return 2;
+    const int lo = pw < ph ? pw : ph, hi = pw < ph ? ph : pw;
+    return hi <= 16 ? 0 : (2 * lo >= hi ? 1 : 2);
+}
+
 // Up to 8 candidates four at a time, lane i (< n) owns candidate i and gets its result: per pass, lanes 0-3 hold the pass's
 // candidates and `eval(m, qx, qy)` returns the distortion of candidate i (< m <= 4) in lane i.
 template <typename F>
@@ -1657,7 +1667,8 @@ __global__ void __launch_bounds__(256, PHASE == 2 ? ME_P2_BLOCKS : (CLS == 1 ? M
     extern __shared__ unsigned char me_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     MeShared* sm = (MeShared*)me_smem + warp;
-    // with `list`: the jobs are list[0 .. *list_n) (the leftovers of the shared-memory-window search, me_window.cuh)
+    // with `list`: the jobs are list[0 .. *list_n) (me_window.cuh: the leftovers of the per-cell pre-checks and of the
+    // shared-memory-window search, the AMP parts that the per-group sub-pel kernels leave)
     if (list) n = *list_n;
     for (;;)
     {
@@ -1717,7 +1728,7 @@ struct MeWinLaunch
     int amp;                                                // AMP partitions present (13 PUs per CU instead of 5): sizes the CTAs
     const int32_t* order;                                   // the slice's jobs sorted by PU shape (absolute indices) or NULL
     int* left_count; int32_t* left_list;
-    int subpelCells;                                        // the class-0 sub-pel jobs of the cells run k_me_subpel_cell (hpel-SATD workloads)
+    int subpelCells;                                        // sub-pel refinement per group: k_me_subpel_cell, k_me_subpel_group (hpel-SATD workloads)
 };
 template <typename P>
 static int launch_me_window(x265cu_ctx* ctx, const void* fenc, int fstride, const uint16_t* mvcost, const x265cu_me_job* jobs,
@@ -1729,6 +1740,11 @@ template <typename P>
 static int launch_me_subpel_cells(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
                                   const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
                                   const MeWinLaunch& w);
+template <typename P>
+static int launch_me_subpel_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
+                                   const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
+                                   const MeWinLaunch& w);
+static int launch_me_subpel_rest(x265cu_ctx* ctx, const x265cu_me_job* jobs, int n, const int32_t* order, int order0, const MeWinLaunch& w);
 
 // Quarter-pel phase planes of the references (the frame analyser, analyser.cuh): every reference is one block of 16 planes
 // `ppitch` elements apart with the reference's stride and origin; slot yf * 4 + xf holds the luma plane interpolated at
@@ -1785,11 +1801,24 @@ static int launch_me_t(x265cu_ctx* ctx, const void* fenc, int fstride, const voi
     // the phase planes are built inside the sub-pel phase, so its time includes them
     const ptrdiff_t pp = planes && !lowres ? planes->ppitch : 0;
     if (pp) rc |= me_build_planes<P>(ctx, *planes);
-    // every class-0 job belongs to a 16x16 cell (the CU 64 / CU 32 groups hold only class-1 PUs): with the cell kernel the
-    // per-PU class-0 launch has nothing left to do
-    if (grp && pp && win->subpelCells) rc |= launch_me_subpel_cells<P>(ctx, fenc, fstride, refs, rstride, pp, ch, mvcost, jobs, st, out, *win);
-    else rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0, pp);
-    rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0, pp);
+    if (grp && pp && win->subpelCells)
+    {
+        // per group, each distinct candidate position once: the 2Nx2N / 2NxN / Nx2N PUs of the CUs 64 and 32, then the class-0
+        // PUs of the 16x16 cells.  Only AMP parts are left for the per-PU class-1 launch, as a job list (the leftover list is
+        // free after the integer search); without AMP there is nothing to launch.
+        rc |= launch_me_subpel_groups<P>(ctx, fenc, fstride, refs, rstride, pp, ch, mvcost, jobs, st, out, *win);
+        rc |= launch_me_subpel_cells<P>(ctx, fenc, fstride, refs, rstride, pp, ch, mvcost, jobs, st, out, *win);
+        if (win->amp)
+        {
+            rc |= launch_me_subpel_rest(ctx, jobs, n, ord, ord0, *win);
+            rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, left, left_n, NULL, 0, pp);
+        }
+    }
+    else
+    {
+        rc |= launch_me_phase<P, 3, 0>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 3, NULL, NULL, ord, ord0, pp);
+        rc |= launch_me_phase<P, 3, 1>(ctx, fenc, fstride, refs, rstride, lowres, ch, mvcost, jobs, n, out, st, counter_dev + 4, NULL, NULL, ord, ord0, pp);
+    }
     return rc;
 }
 

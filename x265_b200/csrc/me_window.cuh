@@ -979,68 +979,19 @@ __device__ __forceinline__ int mec_find(const MeSubTab& t, int E, int it, int sh
     return lo;
 }
 
-template <typename P, bool CHROMA>
-__global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, ptrdiff_t ppitch,
-                                                        MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs,
-                                                        const MeGroup* __restrict__ groups, int ngroups, const int32_t* __restrict__ grp_jobs, int job0,
-                                                        const MeState* __restrict__ state, int32_t* __restrict__ out)
+// me_phase3's stage machine (hpel-SATD workloads: SATD at the start point, half-pel rounds, quarter-pel rounds) of the jobs
+// of one group, one lane per job (`mine`), shared by the per-cell and the per-CU kernels.  Per step the lanes' candidate
+// positions are de-duplicated on (qx, qy) into t.qx / t.qy (at most MEC_NP at a time: a step with more is evaluated in
+// chunks) and t.mask[e] collects the OR of the askers' coverage `mask`; `eval(E)` evaluates entries 0 .. E - 1 over their
+// masks, `dist(e)` returns this lane's distortion at entry e.  Each job starts from `st` as me_phase3 does, tests its own
+// qminy / qmaxy, adds its mvcost and folds its candidates in direction order with ties to the earliest (me_argmin).
+template <typename Tab, typename Eval, typename Dist>
+__device__ __forceinline__ void me_subpel_lanes(Tab& t, int lane, bool mine, const x265cu_me_job& j, int mask, const MeState& st,
+                                                const uint16_t* __restrict__ mvcost, int32_t* __restrict__ o, Eval eval, Dist dist)
 {
-    __shared__ __align__(16) MeSubTab tabs[8];
     const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int gi = blockIdx.x * 8 + warp;
-    if (gi >= ngroups) return;
-    const MeGroup g = groups[gi];
-    MeSubTab& t = tabs[warp];
-
-    // ---- the cell's class-0 jobs, one per lane, in group order (members lane and lane + 32: a cell holds up to 33 jobs) ----
-    int nj;
-    {
-        int m[2]; bool small[2];
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-        {
-            const int i = lane + 32 * h;
-            m[h] = i < g.count ? grp_jobs[g.first + i] - job0 : 0;
-            const int pw = jobs[m[h]].pw, ph = jobs[m[h]].ph;
-            small[h] = i < g.count && !((pw & (pw - 1)) | (ph & (ph - 1))) && pw <= 16 && ph <= 16;
-        }
-        const unsigned b0 = __ballot_sync(FULL, small[0]), b1 = __ballot_sync(FULL, small[1]);
-        const unsigned lt = (1u << lane) - 1u;
-        // the analyser launches this kernel only when every cell has at most 32 of them (an_build_geometry)
-        if (small[0]) t.qx[__popc(b0 & lt)] = m[0];
-        if (small[1]) t.qx[__popc(b0) + __popc(b1 & lt)] = m[1];
-        nj = __popc(b0) + __popc(b1);
-    }
-    __syncwarp();
-    const bool mine = lane < nj;
-    const int jid = mine ? t.qx[lane] : grp_jobs[g.first] - job0;
-    __syncwarp();
-    const x265cu_me_job j = jobs[jid];
-    const int py = j.offset / fstride, px = j.offset - py * fstride;
-    const int cx = __shfl_sync(FULL, px, 0) & ~15, cy = __shfl_sync(FULL, py, 0) & ~15;
-    const ptrdiff_t coff = (ptrdiff_t)cy * fstride + cx;
-    const P* rb = refs[j.ref] + coff;                              // every job of a group has the same reference
-    const P* fb = fenc + coff;
-
-    // per job: its 4x4 tiles inside the cell, its units and chroma tiles, and me_phase3's start
-    const int bx0 = (px - cx) >> 2, by0 = (py - cy) >> 2, bw = j.pw >> 2, bh = j.ph >> 2;
-    const bool chromaOn = CHROMA && j.subme > 2 && !(j.pw & 7) && !(j.ph & 7);           // me_set_chroma
-    int mask = 0;
-    {
-        const int segs = (1 << (((bx0 + bw - 1) >> 1) + 1)) - (1 << (bx0 >> 1));
-        for (int y = by0; y < by0 + bh; y++) mask |= segs << (2 * y);
-        if (chromaOn)
-        {
-            const int tx0 = bx0 >> 1, ty0 = by0 >> 1, tw = j.pw >> 3, th = j.ph >> 3;
-            int cm = 0;
-            for (int y = ty0; y < ty0 + th; y++) for (int x = tx0; x < tx0 + tw; x++) cm |= 1 << (y * 2 + x);
-            mask |= (cm | (cm << 4)) << 8;
-        }
-    }
     const int qminy = j.mvmin[1] * 4, qmaxy = j.mvmax[1] * 4, mvpx = j.qmvp[0], mvpy = j.qmvp[1];
     const int8_t* wl = c_workload[j.subme];
-    const MeState st = state[jid];
     int bcost = st.bcost, bx, by;
     if (st.bprecost < bcost) { bx = st.bestprex; by = st.bestprey; bcost = st.bprecost; }
     else { bx = st.bmx * 4; by = st.bmy * 4; }
@@ -1061,7 +1012,7 @@ __global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fe
         int best = bcost, bdir = 0;
         for (int i0 = 0; i0 < ndir;)
         {
-            // ---- 1. requests of candidates i0 .. i1 - 1, deduplicated on (qx, qy), while the table has room ----
+            // ---- requests of candidates i0 .. i1 - 1, deduplicated on (qx, qy), while the table has room ----
             int E = 0, i1 = i0;
             for (; i1 < ndir; i1++)
             {
@@ -1089,7 +1040,97 @@ __global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fe
                 }
             }
             __syncwarp();
-            // ---- 2. prefix of the entries' unit and tile counts ----
+            eval(E);
+            __syncwarp();
+            // ---- each job folds its candidates i0 .. i1 - 1 in order (me_argmin: ties to the earliest) ----
+            for (int i = i0; i < i1; i++)
+            {
+                const int e = (int)(((i < 4 ? sl0 : sl1) >> (8 * (i & 3))) & 0xffu);
+                if (e == 0xff) continue;
+                const int d1 = centre ? 0 : i + 1;
+                const int qx = bx + c_square1[d1][0] * step, qy = by + c_square1[d1][1] * step;
+                const int cost = dist(e) + me_mvcost(mvcost, mvpx, mvpy, qx, qy);
+                if (centre) best = cost;
+                else if (cost < best) { best = cost; bdir = d1; }
+            }
+            __syncwarp();
+            i0 = i1;
+        }
+        // ---- the next stage, as me_phase3 ----
+        if (live)
+        {
+            if (centre) { bcost = best; stage = 1; }
+            else if (bdir) { bcost = best; bx += c_square1[bdir][0] * step; by += c_square1[bdir][1] * step; it++; }
+            else if (stage == 1) { stage = 3; it = 0; }
+            else live = false;
+        }
+    }
+    if (mine) { o[0] = bcost; o[1] = bx; o[2] = by; o[3] = 0; }
+}
+
+template <typename P, bool CHROMA>
+__global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, ptrdiff_t ppitch,
+                                                        MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs,
+                                                        const MeGroup* __restrict__ groups, int ngroups, const int32_t* __restrict__ grp_jobs, int job0,
+                                                        const MeState* __restrict__ state, int32_t* __restrict__ out)
+{
+    __shared__ __align__(16) MeSubTab tabs[8];
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gi = blockIdx.x * 8 + warp;
+    if (gi >= ngroups) return;
+    const MeGroup g = groups[gi];
+    MeSubTab& t = tabs[warp];
+
+    // ---- the cell's class-0 jobs, one per lane, in group order (members lane and lane + 32: a cell holds up to 33 jobs) ----
+    int nj;
+    {
+        int m[2]; bool small[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+        {
+            const int i = lane + 32 * h;
+            m[h] = i < g.count ? grp_jobs[g.first + i] - job0 : 0;
+            small[h] = i < g.count && me_subpel_kernel(jobs[m[h]].pw, jobs[m[h]].ph) == 0;
+        }
+        const unsigned b0 = __ballot_sync(FULL, small[0]), b1 = __ballot_sync(FULL, small[1]);
+        const unsigned lt = (1u << lane) - 1u;
+        // the analyser launches this kernel only when every cell has at most 32 of them (an_build_geometry)
+        if (small[0]) t.qx[__popc(b0 & lt)] = m[0];
+        if (small[1]) t.qx[__popc(b0) + __popc(b1 & lt)] = m[1];
+        nj = __popc(b0) + __popc(b1);
+    }
+    __syncwarp();
+    const bool mine = lane < nj;
+    const int jid = mine ? t.qx[lane] : grp_jobs[g.first] - job0;
+    __syncwarp();
+    const x265cu_me_job j = jobs[jid];
+    const int py = j.offset / fstride, px = j.offset - py * fstride;
+    const int cx = __shfl_sync(FULL, px, 0) & ~15, cy = __shfl_sync(FULL, py, 0) & ~15;
+    const ptrdiff_t coff = (ptrdiff_t)cy * fstride + cx;
+    const P* rb = refs[j.ref] + coff;                              // every job of a group has the same reference
+    const P* fb = fenc + coff;
+
+    // per job: its 4x4 tiles inside the cell, its units and chroma tiles
+    const int bx0 = (px - cx) >> 2, by0 = (py - cy) >> 2, bw = j.pw >> 2, bh = j.ph >> 2;
+    const bool chromaOn = CHROMA && j.subme > 2 && !(j.pw & 7) && !(j.ph & 7);           // me_set_chroma
+    int mask = 0;
+    {
+        const int segs = (1 << (((bx0 + bw - 1) >> 1) + 1)) - (1 << (bx0 >> 1));
+        for (int y = by0; y < by0 + bh; y++) mask |= segs << (2 * y);
+        if (chromaOn)
+        {
+            const int tx0 = bx0 >> 1, ty0 = by0 >> 1, tw = j.pw >> 3, th = j.ph >> 3;
+            int cm = 0;
+            for (int y = ty0; y < ty0 + th; y++) for (int x = tx0; x < tx0 + tw; x++) cm |= 1 << (y * 2 + x);
+            mask |= (cm | (cm << 4)) << 8;
+        }
+    }
+
+    me_subpel_lanes(t, lane, mine, j, mask, state[jid], mvcost, out + (size_t)jid * 4,
+        [&](int E)
+        {
+            // ---- prefix of the entries' unit and tile counts ----
             int total = 0;
             for (int e0 = 0; e0 < E; e0 += 32)
             {
@@ -1103,7 +1144,7 @@ __global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fe
                 total += __shfl_sync(FULL, v, 31);
             }
             __syncwarp();
-            // ---- 3. luma: 8 units per pass, a unit's 4 rows on 4 consecutive lanes (me_seg_cost's butterflies) ----
+            // ---- luma: 8 units per pass, a unit's 4 rows on 4 consecutive lanes (me_seg_cost's butterflies) ----
             const int nu = total & 0xffff, nt = total >> 16;
             for (int u0 = 0; u0 < nu; u0 += 8)
             {
@@ -1145,7 +1186,7 @@ __global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fe
                 for (int s = 1; s <= 2; s <<= 1) { sl += __shfl_xor_sync(FULL, sl, s); sr += __shfl_xor_sync(FULL, sr, s); }
                 if (on && row == 0) { int* L = &t.lum[e][(unit >> 1) * 4 + (unit & 1) * 2]; L[0] = sl; L[1] = sr; }
             }
-            // ---- 4. chroma: one lane per (position, plane, tile) ----
+            // ---- chroma: one lane per (position, plane, tile) ----
             if (CHROMA)
                 for (int c0 = 0; c0 < nt; c0 += 32)
                 {
@@ -1161,53 +1202,163 @@ __global__ void __launch_bounds__(256) k_me_subpel_cell(const P* __restrict__ fe
                         t.chr[e][k] = me_chroma_had4x4<P>(f, r, ch.cstride, qx & 7, qy & 7);
                     }
                 }
-            __syncwarp();
-            // ---- 5. each job folds its candidates i0 .. i1 - 1 in order (me_argmin: ties to the earliest) ----
-            for (int i = i0; i < i1; i++)
-            {
-                const int e = (int)(((i < 4 ? sl0 : sl1) >> (8 * (i & 3))) & 0xffu);
-                if (e == 0xff) continue;
-                const int d1 = centre ? 0 : i + 1;
-                const int qx = bx + c_square1[d1][0] * step, qy = by + c_square1[d1][1] * step;
-                const int* L = t.lum[e];
-                int cost = 0;
-                for (int y = by0; y < by0 + bh; y++)
-                {
-                    if (bw == 1) cost += L[y * 4 + bx0] >> 1;
-                    else for (int x = bx0; x < bx0 + bw; x += 2) cost += (L[y * 4 + x] + L[y * 4 + x + 1]) >> 1;
-                }
-                if (chromaOn)
-                {
-                    const int tx0 = bx0 >> 1, ty0 = by0 >> 1, th = j.ph >> 3;
-#pragma unroll
-                    for (int cr = 0; cr < 2; cr++)
-                        for (int y = ty0; y < ty0 + th; y++)
-                        {
-                            const int* s = &t.chr[e][cr * 4 + y * 2];
-                            cost += j.pw == 16 ? (s[0] + s[1]) >> 1 : s[tx0] >> 1;
-                        }
-                }
-                cost += me_mvcost(mvcost, mvpx, mvpy, qx, qy);
-                if (centre) best = cost;
-                else if (cost < best) { best = cost; bdir = d1; }
-            }
-            __syncwarp();
-            i0 = i1;
-        }
-        // ---- 6. the next stage, as me_phase3 ----
-        if (live)
+        },
+        [&](int e)
         {
-            if (centre) { bcost = best; stage = 1; }
-            else if (bdir) { bcost = best; bx += c_square1[bdir][0] * step; by += c_square1[bdir][1] * step; it++; }
-            else if (stage == 1) { stage = 3; it = 0; }
-            else live = false;
-        }
+            const int* L = t.lum[e];
+            int cost = 0;
+            for (int y = by0; y < by0 + bh; y++)
+            {
+                if (bw == 1) cost += L[y * 4 + bx0] >> 1;
+                else for (int x = bx0; x < bx0 + bw; x += 2) cost += (L[y * 4 + x] + L[y * 4 + x + 1]) >> 1;
+            }
+            if (chromaOn)
+            {
+                const int tx0 = bx0 >> 1, ty0 = by0 >> 1, th = j.ph >> 3;
+#pragma unroll
+                for (int cr = 0; cr < 2; cr++)
+                    for (int y = ty0; y < ty0 + th; y++)
+                    {
+                        const int* s = &t.chr[e][cr * 4 + y * 2];
+                        cost += j.pw == 16 ? (s[0] + s[1]) >> 1 : s[tx0] >> 1;
+                    }
+            }
+            return cost;
+        });
+}
+
+// ---- sub-pel refinement of the CU 64 / CU 32 groups --------------------------------------------------------------------
+// The same sharing one level up.  The five PUs of a CU (2Nx2N, 2 x 2NxN, 2 x Nx2N) cover it three times; on the same
+// integer vector they ask for the same half-pel and quarter-pel positions.  One warp runs the stage machine of a CU's PUs
+// (me_subpel_lanes, one lane per PU) and evaluates each distinct position once per 32x32 quadrant the askers cover (a CU 32
+// is one quadrant): the quadrant's 32 luma 8x4 units are one warp pass, the whole Hadamard in the lane as in
+// me_subpel_big, and its 2 x 16 chroma 4x4 tiles are one pass of me_chroma_had4x4.  Every PU side is a multiple of 16, so
+// luma is tiled 8x4 and chroma (widths 8 / 16 / 32) 8x4 for all of them: a lane's unit, and a lane pair's chroma tile, is a
+// whole tile of every PU that covers it, and a PU's SATD is the sum of the lanes it covers.  Coverage is kept per 16x16
+// block of the CU (a 4x4 grid of bits; 2x2 used by a CU 32).  The CUs' AMP parts stay with the per-PU class-1 launch.
+struct MeGrpTab
+{
+    int qx[MEC_NP], qy[MEC_NP];
+    int mask[MEC_NP];                      // bits 0-15: 16x16 blocks (row * 4 + column) asked for in luma; 16-31: in chroma
+    int dist[MEC_NP][8];                   // per job slot (a CU has five such PUs): luma + chroma SATD at the entry
+};
+
+template <typename P, bool CHROMA>
+__global__ void __launch_bounds__(256, 2) k_me_subpel_group(const P* __restrict__ fenc, int fstride, const P* const* __restrict__ refs, int rstride, ptrdiff_t ppitch,
+                                                            MeChromaArgs ch, const uint16_t* __restrict__ mvcost, const x265cu_me_job* __restrict__ jobs,
+                                                            const MeGroup* __restrict__ groups64, int n64, const int32_t* __restrict__ grp_jobs64,
+                                                            const MeGroup* __restrict__ groups32, int n32, const int32_t* __restrict__ grp_jobs32, int job0,
+                                                            const MeState* __restrict__ state, int32_t* __restrict__ out)
+{
+    __shared__ __align__(16) MeGrpTab tabs[8];
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // the CU 64 groups (four times the work) first, so that they do not form the tail of the launch
+    const int gi = blockIdx.x * 8 + warp;
+    if (gi >= n64 + n32) return;
+    const bool big = gi < n64;
+    const MeGroup g = big ? groups64[gi] : groups32[gi - n64];
+    const int32_t* grp_jobs = big ? grp_jobs64 : grp_jobs32;
+    MeGrpTab& t = tabs[warp];
+
+    // ---- the CU's 2Nx2N / 2NxN / Nx2N jobs, one per lane, in group order (a group holds up to 13 jobs with AMP) ----
+    int nj;
+    {
+        const int m = lane < g.count ? grp_jobs[g.first + lane] - job0 : 0;
+        const bool take = lane < g.count && me_subpel_kernel(jobs[m].pw, jobs[m].ph) == 1;
+        const unsigned b = __ballot_sync(FULL, take);
+        if (take) t.qx[__popc(b & ((1u << lane) - 1u))] = m;
+        nj = __popc(b);
     }
-    if (mine) { int32_t* o = out + (size_t)jid * 4; o[0] = bcost; o[1] = bx; o[2] = by; o[3] = 0; }
+    __syncwarp();
+    const bool mine = lane < nj;
+    const int jid = mine ? t.qx[lane] : grp_jobs[g.first] - job0;
+    __syncwarp();
+    const x265cu_me_job j = jobs[jid];
+    const int py = j.offset / fstride, px = j.offset - py * fstride;
+    const int edge = big ? 64 : 32;
+    const int cx = __shfl_sync(FULL, px, 0) & ~(edge - 1), cy = __shfl_sync(FULL, py, 0) & ~(edge - 1);
+    const ptrdiff_t coff = (ptrdiff_t)cy * fstride + cx;
+    const P* rb = refs[j.ref] + coff;                              // every job of a group has the same reference
+    const P* fb = fenc + coff;
+    const ptrdiff_t coffC = CHROMA ? (ptrdiff_t)(cy >> 1) * ch.cstride + (cx >> 1) : 0;
+
+    int mask = 0;
+    for (int y = (py - cy) >> 4; y < (py - cy + j.ph) >> 4; y++)
+        for (int x = (px - cx) >> 4; x < (px - cx + j.pw) >> 4; x++) mask |= 1 << (y * 4 + x);
+    if (CHROMA && j.subme > 2) mask |= mask << 16;                 // me_set_chroma: the sides are multiples of 8
+    if (!mine) mask = 0;
+
+    // my 8x4 luma unit of a quadrant: column lane & 3, row lane >> 2; my chroma tile: plane (lane >> 2) & 1, column lane & 3,
+    // row lane >> 3 -- so that both lie in the quadrant's 16x16 block ((lane >> 1) & 1, lane >> 4)
+    const int ux = lane & 3, uy = lane >> 2, blk = (lane >> 4) * 4 + ((lane >> 1) & 1);
+    const int cty = lane >> 3;
+    const bool cr = (lane >> 2) & 1;
+    const P* fC = (const P*)(cr ? ch.fencCr : ch.fencCb) + coffC;
+    const P* rC = CHROMA ? ((const P* const*)(cr ? ch.refCr : ch.refCb))[j.ref] + coffC : nullptr;
+
+    me_subpel_lanes(t, lane, mine, j, mask, state[jid], mvcost, out + (size_t)jid * 4,
+        [&](int E)
+        {
+            for (int e = 0; e < E; e++)
+            {
+                const int m = t.mask[e], qx = t.qx[e], qy = t.qy[e];
+                const P* r0 = rb + (qx >> 2) + (ptrdiff_t)(qy >> 2) * rstride + ((qy & 3) * 4 + (qx & 3)) * ppitch;
+                int acc = 0;
+                for (int q = 0; q < (big ? 4 : 1); q++)
+                {
+                    const int X0 = (q & 1) * 2, Y0 = (q >> 1) * 2;         // the quadrant's first 16x16 block
+                    if (!((m | (m >> 16)) & (0x33 << (Y0 * 4 + X0)))) continue;
+                    const int bit = Y0 * 4 + X0 + blk;
+                    int lum = 0, chr = 0;
+                    if ((m >> bit) & 1)
+                    {   // one 8x4 tile (pixel.cpp:239-261): two 4x4 Hadamards, halved together
+                        const int x = X0 * 16 + ux * 8, y = Y0 * 16 + uy * 4;
+                        int d[4][8];
+#pragma unroll
+                        for (int k = 0; k < 4; k++)
+                        {
+                            int fv[8];
+                            me_load_row8<P>(r0 + (ptrdiff_t)(y + k) * rstride + x, d[k]);
+                            me_load_row8<P>(fb + (ptrdiff_t)(y + k) * fstride + x, fv);
+#pragma unroll
+                            for (int i = 0; i < 8; i++) d[k][i] = fv[i] - d[k][i];
+                            had4(d[k][0], d[k][1], d[k][2], d[k][3]); had4(d[k][4], d[k][5], d[k][6], d[k][7]);
+                        }
+#pragma unroll
+                        for (int i = 0; i < 8; i++)
+                        {
+                            had4(d[0][i], d[1][i], d[2][i], d[3][i]);
+                            lum += abs(d[0][i]) + abs(d[1][i]) + abs(d[2][i]) + abs(d[3][i]);
+                        }
+                        lum >>= 1;
+                    }
+                    if (CHROMA)
+                    {
+                        if ((m >> (16 + bit)) & 1)
+                        {
+                            const ptrdiff_t o = (ptrdiff_t)(Y0 * 8 + cty * 4) * ch.cstride + X0 * 8 + ux * 4;
+                            chr = me_chroma_had4x4<P>(fC + o, rC + o + (qx >> 3) + (ptrdiff_t)(qy >> 3) * ch.cstride, ch.cstride, qx & 7, qy & 7);
+                        }
+                        // 8x4 chroma tiles: the two 4x4 sums of a lane pair added and halved, kept by the even lane
+                        chr += __shfl_xor_sync(FULL, chr, 1);
+                        chr = (lane & 1) ? 0 : chr >> 1;
+                    }
+                    for (int s = 0; s < nj; s++)
+                    {
+                        const int jm = __shfl_sync(FULL, mask, s);
+                        const int v = __reduce_add_sync(FULL, (((jm >> bit) & 1) ? lum : 0) + (((jm >> (16 + bit)) & 1) ? chr : 0));
+                        if (lane == s) acc += v;
+                    }
+                }
+                if (mine) t.dist[e][lane] = acc;
+            }
+        },
+        [&](int e) { return t.dist[e][lane]; });
 }
 
 // Sub-pel refinement of the class-0 jobs of a frame slice's 16x16 cells (k_me_subpel_cell), on the phase planes `ppitch`
-// elements apart; the per-PU class-1 launch takes every other job.
+// elements apart.
 template <typename P>
 static int launch_me_subpel_cells(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
                                   const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
@@ -1218,6 +1369,46 @@ static int launch_me_subpel_cells(x265cu_ctx* ctx, const void* fenc, int fstride
     const auto kernel = ch ? k_me_subpel_cell<P, true> : k_me_subpel_cell<P, false>;
     kernel<<<(w.ngroups[2] + 7) / 8, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ppitch, ch ? *ch : none, mvcost, jobs,
                                                            (const MeGroup*)w.groups[2], w.ngroups[2], w.grp_jobs[2], w.job0, st, out);
+    CU_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// Sub-pel refinement of the 2Nx2N / 2NxN / Nx2N jobs of a frame slice's CU 64 and CU 32 groups (k_me_subpel_group)
+template <typename P>
+static int launch_me_subpel_groups(x265cu_ctx* ctx, const void* fenc, int fstride, const void* const* refs, int rstride, ptrdiff_t ppitch,
+                                   const MeChromaArgs* ch, const uint16_t* mvcost, const x265cu_me_job* jobs, const MeState* st, int32_t* out,
+                                   const MeWinLaunch& w)
+{
+    const int n = w.ngroups[0] + w.ngroups[1];
+    if (n <= 0) return 0;
+    const MeChromaArgs none = {};
+    const auto kernel = ch ? k_me_subpel_group<P, true> : k_me_subpel_group<P, false>;
+    kernel<<<(n + 7) / 8, 256, 0, ctx->stream>>>((const P*)fenc, fstride, (const P* const*)refs, rstride, ppitch, ch ? *ch : none, mvcost, jobs,
+                                                 (const MeGroup*)w.groups[0], w.ngroups[0], w.grp_jobs[0], (const MeGroup*)w.groups[1], w.ngroups[1],
+                                                 w.grp_jobs[1], w.job0, st, out);
+    CU_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// The jobs of a launch slice that neither of the two kernels above refines (AMP parts), appended to `left_list` in the
+// order of `order` (NULL: job order) for the per-PU class-1 launch
+__global__ void __launch_bounds__(256) k_me_subpel_rest(const x265cu_me_job* __restrict__ jobs, int n, const int32_t* __restrict__ order, int order0,
+                                                        int* __restrict__ left_count, int32_t* __restrict__ left_list)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x, lane = threadIdx.x & 31;
+    const int jid = i >= n ? 0 : order ? order[i] - order0 : i;
+    const bool keep = i < n && me_subpel_kernel(jobs[jid].pw, jobs[jid].ph) == 2;
+    const unsigned b = __ballot_sync(0xffffffffu, keep);
+    int base = 0;
+    if (b && lane == 0) base = atomicAdd(left_count, __popc(b));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (keep) left_list[base + __popc(b & ((1u << lane) - 1u))] = jid;
+}
+
+static int launch_me_subpel_rest(x265cu_ctx* ctx, const x265cu_me_job* jobs, int n, const int32_t* order, int order0, const MeWinLaunch& w)
+{
+    CU_CHECK(cudaMemsetAsync(w.left_count, 0, sizeof(int), ctx->stream));
+    k_me_subpel_rest<<<(n + 255) / 256, 256, 0, ctx->stream>>>(jobs, n, order, order0, w.left_count, w.left_list);
     CU_LAUNCH_CHECK(ctx);
     return 0;
 }
