@@ -297,6 +297,10 @@ int x265cu_analyser_ref_chroma_updated(x265cu_analyser*, int idx);     /* re-ext
 /* device address of chroma plane `plane` (0 Cb, 1 Cr) of ref idx at pixel (0,0) and its stride in elements (NULL before
  * enable_chroma()); the chroma twin of x265cu_analyser_ref_plane */
 void* x265cu_analyser_ref_plane_chroma(x265cu_analyser*, int idx, int plane, int* cstride);
+/* device address of the resident source plane `plane` (0 luma, 1 Cb, 2 Cr) at pixel (0,0) and its stride in elements, as
+ * the last load_inputs() / load_chroma() left it (NULL for chroma before enable_chroma()); the source twin of ref_plane /
+ * ref_plane_chroma, e.g. for x265cu_sao_stats_frame */
+void* x265cu_analyser_src_plane(x265cu_analyser*, int plane, int* stride);
 
 /* ---------- frame-level deblocking (common/deblock.cpp) ----------
  * The host's final decisions, one record per 4x4 luma unit in raster order over the picture (width / 4 records per row),
@@ -330,6 +334,43 @@ typedef struct {
  * unspecified pixels, never a fault. */
 int x265cu_deblock_frame(x265cu_ctx*, int depth, void* luma_dev, int stride, void* cb_dev, void* cr_dev, int cstride,
                          int width, int height, const x265cu_deblock_unit* units_dev, const x265cu_deblock_params* params);
+
+/* ---------- frame-level SAO (encoder/sao.cpp): statistics and apply; the decision stays on the host ----------
+ * One slice per picture; 4:2:0, or 4:0:0 when every chroma pointer is NULL; CTU 16, 32 or 64.  Planes are device pointers at
+ * pixel (0,0), strides in elements; both calls run on the context's stream.  Both read the deblocked, not-yet-SAO'd
+ * picture only, as FrameFilter's interleaved order does (the statistics skip the samples the next CTU row's deblocking still
+ * changes; the apply of a CTU reads its neighbours from copies taken before any SAO), so a picture is: x265cu_deblock_frame,
+ * x265cu_sao_stats_frame, the host's SAO decision, x265cu_sao_apply_frame.  Each call returns -1 with x265cu_last_error(),
+ * before any launch, for depth not 8 or 10, width or height not a positive multiple of 8, another CTU size, a stride smaller
+ * than the row, a NULL luma / stats / parameter pointer, only some chroma pointers, saoChroma without chroma planes, flags
+ * other than 0 or 1, or bypass units without source planes. */
+typedef struct {
+    int8_t  typeIdx;        /* SaoCtuParam as rdoSaoUnitCu leaves it (merged CTUs hold the copied parameters): -1 off,
+                               0..3 SAO_EO_0..3, 4 SAO_BO; any other value is off */
+    uint8_t bandPos;        /* 0..31, read & 31 */
+    int8_t  offset[4];      /* any value: the result is clipped to the pixel range */
+    uint8_t pad[2];
+} x265cu_sao_ctu;           /* 8 bytes; arrays [3][numCtus], CTU raster order */
+
+/* SAO::calcSaoStatsCTU of every CTU and plane (sao.cpp:735-917), all five types (bLimitSAO is the caller's: INTEGRATION.md).
+ * stats_dev: int32 [numCtus][2: count, offsetOrg][3][5][32], i.e. two SAO::PerPlane per CTU (types in SaoType order, edge
+ * classes through s_eoTable), ready to memcpy into m_count / m_offsetOrg.  Every entry is written; entries the reference never
+ * writes (classes >= 5 of the edge types, chroma of a 4:0:0 call) are 0. */
+int x265cu_sao_stats_frame(x265cu_ctx*, int depth, int width, int height, int ctuSize,
+                           const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                           const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats_dev);
+
+/* FrameFilter's processSaoCTU over every CTU (generateLumaOffsets / generateChromaOffsets / applyPixelOffsets, sao.cpp:274-732),
+ * in place.  saoLuma / saoChroma: SAOParam::bSaoFlag[0 / 1].  Cr is filtered with Cb's type and its own offsets, and only
+ * when both types are >= 0 (sao.cpp:727; x265's decision gives both the same type; an EO record of one and a BO record of the
+ * other give unspecified Cr pixels).  bypass_units_dev: NULL, or the x265cu_deblock_unit map, whose transquant-bypass units
+ * (flags bit 2) then get the source samples back (origCUSampleRestoration).  Out-of-range records give unspecified pixels,
+ * never a fault. */
+int x265cu_sao_apply_frame(x265cu_ctx*, int depth, int width, int height, int ctuSize,
+                           void* y, void* cb, void* cr, int stride, int cstride,
+                           const x265cu_sao_ctu* params_dev, int saoLuma, int saoChroma,
+                           const x265cu_deblock_unit* bypass_units_dev,
+                           const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride);
 
 /* ---------- lookahead frame costs (BASELINE configs[1]; slicetype.cpp:696-805, 3115-3388) ----------
  * All pointers are device pointers.  Planes are the 4 lowres hpel planes of a frame (origin pixel,

@@ -641,6 +641,16 @@ void* x265cu_analyser_ref_plane_chroma(x265cu_analyser* a, int idx, int plane, i
     return a->d_refC[idx][plane] + a->cOrgBytes;
 }
 
+// device address of source plane `plane` (0 luma, 1 Cb, 2 Cr) at its origin pixel and its stride in elements: the twin of
+// ref_plane / ref_plane_chroma for the calls that read the source, e.g. x265cu_sao_stats_frame
+void* x265cu_analyser_src_plane(x265cu_analyser* a, int plane, int* stride)
+{
+    if (plane == 0) { *stride = a->stride; return a->d_fenc + a->orgBytes; }
+    if (!a->chromaOn || plane < 0 || plane > 2) return NULL;
+    *stride = a->cstride;
+    return a->d_fencC[plane - 1] + a->cOrgBytes;
+}
+
 int x265cu_analyser_run_resident(x265cu_analyser* a, int stages) { return an_run(a, stages, 0, a->ctuRows); }
 
 // ---- CTU-row shards (the WPP row partition of SURVEY 8(e): frameencoder.cpp:850-868 enables row r once the

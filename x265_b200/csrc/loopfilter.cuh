@@ -480,4 +480,293 @@ __global__ void k_sao_stats_e3(const int16_t* __restrict__ diff, const P* __rest
     stats_flush<5>(s_st, s_ct, stats, count, true);
 }
 
+// ---- frame-level SAO (x265cu_sao_stats_frame / x265cu_sao_apply_frame): whole planes, one CTA per (CTU, plane) ----
+// Both read the deblocked, not-yet-SAO'd picture only (include/x265_b200.h; pinned by tests/test_sao_oracle_vs_ref.py).
+
+// the edge class of sample c between its neighbours a and b (edgeType of sao.cpp / loopfilter.cpp: 0..4, 2 = neither)
+__device__ __forceinline__ int sao_edge_type(int c, int a, int b) { return sgn(c - a) + sgn(c - b) + 2; }
+// the band of sample c (SAO_BO_BITS = 5)
+template <typename P> __device__ __forceinline__ int sao_band(int c) { return c >> (PixTraits<P>::depth - 5); }
+
+// The geometry of CTU `addr` in plane p (calcSaoStatsCTU / applyPixelOffsets, sao.cpp:274-308, 735-767): origin, size
+// clipped to the picture, and whether it touches each picture border.
+struct SaoCtuGeom
+{
+    int picW, picH, lpelx, tpely, w, h;
+    bool left, top, right, bottom;
+};
+__device__ __forceinline__ SaoCtuGeom sao_ctu_geom(int width, int height, int log2Ctu, int cols, int addr, int p)
+{
+    SaoCtuGeom g;
+    const int s = p ? 1 : 0, log2S = log2Ctu - s;
+    g.picW = width >> s; g.picH = height >> s;
+    g.lpelx = (addr % cols) << log2S; g.tpely = (addr / cols) << log2S;
+    g.w = min(1 << log2S, g.picW - g.lpelx); g.h = min(1 << log2S, g.picH - g.tpely);
+    g.left = g.lpelx == 0; g.top = g.tpely == 0;
+    g.right = g.lpelx + g.w == g.picW; g.bottom = g.tpely + g.h == g.picH;
+    return g;
+}
+
+struct SaoStatsArgs
+{
+    const void* fenc[3]; const void* rec[3];   // at pixel (0,0); planes = 1: luma only
+    int fstride, fcstride, stride, cstride, width, height, log2Ctu, cols, planes;
+    int32_t* stats;                            // [numCtus][2][3][5][32]
+};
+
+// SAO::calcSaoStatsCTU (sao.cpp:735-917) of CTU blockIdx.x, plane blockIdx.y: every sample of the CTU once, classified for
+// each type inside that type's region (skipB 4 / skipR 5 away from the picture's right / bottom border, 2 / 3 in chroma; the
+// E0 rows ignore the picture bottom, sao.cpp:836).  Neighbour coordinates are clamped to the picture: the regions only hold
+// samples whose neighbours lie inside it.  Edge-type counts and sums stay in registers, band histograms in per-warp shared
+// bins; warp reductions, then one sum over the warps.  The CTA writes its plane's whole record (320 entries), zeros included.
+template <typename P>
+__global__ void __launch_bounds__(256) k_sao_stats_frame(const SaoStatsArgs a)
+{
+    constexpr int NW = 8;
+    __shared__ int s_bo[NW][2][32];
+    __shared__ int s_eo[NW][2][4][5];
+    const int addr = blockIdx.x, p = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (int i = tid; i < NW * 2 * 32; i += blockDim.x) (&s_bo[0][0][0])[i] = 0;
+    __syncthreads();
+    int ec[4][5], es[4][5];
+#pragma unroll
+    for (int t = 0; t < 4; t++)
+#pragma unroll
+        for (int k = 0; k < 5; k++) { ec[t][k] = 0; es[t][k] = 0; }
+    if (p < a.planes)
+    {
+        const SaoCtuGeom g = sao_ctu_geom(a.width, a.height, a.log2Ctu, a.cols, addr, p);
+        const int po = p ? 2 : 0, log2S = a.log2Ctu - (p ? 1 : 0), S = 1 << log2S;
+        const int boX = g.right ? g.w : g.w - 5 + po, boY = g.bottom ? g.h : g.h - 4 + po;
+        const int sx = g.left, sy = g.top;
+        const int eX = g.right ? g.w - 1 : g.w - 5 + po, e0Y = g.h - 4 + po, e1Y = g.bottom ? g.h - 1 : g.h - 4 + po;
+        const P* rec = (const P*)(p == 0 ? a.rec[0] : p == 1 ? a.rec[1] : a.rec[2]);     // constant indices: no stack copy
+        const P* fenc = (const P*)(p == 0 ? a.fenc[0] : p == 1 ? a.fenc[1] : a.fenc[2]);
+        const ptrdiff_t rs = p ? a.cstride : a.stride, fs = p ? a.fcstride : a.fstride;
+        for (int i = tid; i < S * S; i += blockDim.x)
+        {
+            const int x = i & (S - 1), y = i >> log2S;
+            const bool inBo = x < boX && y < boY;
+            const bool inE0 = x >= sx && x < eX && y < e0Y;
+            const bool inE1 = x < boX && y >= sy && y < e1Y;
+            const bool inE23 = x >= sx && x < eX && y >= sy && y < e1Y;
+            if (!(inBo || inE0 || inE1 || inE23)) continue;
+            const int px = g.lpelx + x, py = g.tpely + y;
+            const int xl = max(px - 1, 0), xr = min(px + 1, g.picW - 1);
+            const P* r0 = rec + (ptrdiff_t)max(py - 1, 0) * rs;
+            const P* r1 = rec + (ptrdiff_t)py * rs;
+            const P* r2 = rec + (ptrdiff_t)min(py + 1, g.picH - 1) * rs;
+            const int c = r1[px], diff = (int)fenc[(ptrdiff_t)py * fs + px] - c;
+            if (inBo)
+            {
+                const int b = sao_band<P>(c);
+                atomicAdd(&s_bo[warp][0][b], 1);
+                atomicAdd(&s_bo[warp][1][b], diff);
+            }
+            int et[4];
+            et[0] = inE0 ? sao_edge_type(c, r1[xl], r1[xr]) : -1;
+            et[1] = inE1 ? sao_edge_type(c, r0[px], r2[px]) : -1;
+            et[2] = inE23 ? sao_edge_type(c, r0[xl], r2[xr]) : -1;
+            et[3] = inE23 ? sao_edge_type(c, r0[xr], r2[xl]) : -1;
+#pragma unroll
+            for (int t = 0; t < 4; t++)
+#pragma unroll
+                for (int k = 0; k < 5; k++)
+                {
+                    ec[t][k] += et[t] == k;
+                    es[t][k] += et[t] == k ? diff : 0;
+                }
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < 4; t++)
+#pragma unroll
+        for (int k = 0; k < 5; k++)
+        {
+            const int n = warp_sum(ec[t][k]), d = warp_sum(es[t][k]);
+            if (lane == 0) { s_eo[warp][0][t][k] = n; s_eo[warp][1][t][k] = d; }
+        }
+    __syncthreads();
+    // [count / offsetOrg][type][class]: BO classes are bands; edge class k is edgeType eoInv[k] (s_eoTable = {1, 2, 0, 3, 4})
+    int32_t* rec = a.stats + (size_t)addr * (2 * 3 * 5 * 32) + p * (5 * 32);
+    for (int i = tid; i < 2 * 5 * 32; i += blockDim.x)
+    {
+        const int kind = i / (5 * 32), t = (i >> 5) % 5, k = i & 31;
+        int v = 0;
+        if (t == 4)
+            for (int w = 0; w < NW; w++) v += s_bo[w][kind][k];
+        else if (k < 5)
+        {
+            const int e = k == 0 ? 2 : k == 1 ? 0 : k == 2 ? 1 : k;
+            for (int w = 0; w < NW; w++) v += s_eo[w][kind][t][e];
+        }
+        rec[kind * (3 * 5 * 32) + t * 32 + k] = v;
+    }
+}
+
+struct SaoApplyArgs
+{
+    void* plane[3]; const void* fenc[3];       // at pixel (0,0); planes = 1: luma only
+    int stride, cstride, fstride, fcstride, width, height, log2Ctu, cols, rows, planes;
+    int on[3];                                 // SAOParam::bSaoFlag per plane
+    const x265cu_sao_ctu* params;              // [3][numCtus]
+    const x265cu_deblock_unit* units;          // NULL: no transquant-bypass restoration
+    void* lines[3];                            // per plane: [rows][2: top, bottom][picW], then [cols][2: left, right][picH]
+};
+
+// Saves the edge lines of every CTU of the planes with SAO on (the reference's m_tmpU / m_tmpL at picture scope), so that
+// k_sao_apply_frame can filter in place: thread i of plane blockIdx.y copies entry i of that plane's line store.
+template <typename P>
+__global__ void __launch_bounds__(256) k_sao_save_lines(const SaoApplyArgs a)
+{
+    const int p = blockIdx.y;
+    if (p >= a.planes || !a.on[p]) return;
+    const int s = p ? 1 : 0, picW = a.width >> s, picH = a.height >> s, S = 1 << (a.log2Ctu - s);
+    const P* src = (const P*)a.plane[p];
+    const ptrdiff_t st = p ? a.cstride : a.stride;
+    P* dst = (P*)a.lines[p];
+    const long nRow = (long)a.rows * 2 * picW, nAll = nRow + (long)a.cols * 2 * picH;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < nAll; i += (long)gridDim.x * blockDim.x)
+    {
+        int x, y;
+        if (i < nRow)
+        {
+            const int r = (int)(i / (2 * picW)), side = (int)(i / picW) & 1;
+            x = (int)(i % picW);
+            y = side ? min((r + 1) * S, picH) - 1 : r * S;
+        }
+        else
+        {
+            const long j = i - nRow;
+            const int c = (int)(j / (2 * picH)), side = (int)(j / picH) & 1;
+            y = (int)(j % picH);
+            x = side ? min((c + 1) * S, picW) - 1 : c * S;
+        }
+        dst[i] = src[(ptrdiff_t)y * st + x];
+    }
+}
+
+// processSaoCTU of CTU blockIdx.x, plane blockIdx.y (sao.cpp:274-732, framefilter.cpp:324-343), in place: the CTA stages its
+// CTU from the plane and a one-sample ring from the saved lines into shared memory, then writes the filtered samples of its
+// own CTU only.  Which samples a type changes: BO all; EO_0 not the picture's left / right column; EO_1 not its top /
+// bottom row; EO_2 / EO_3 neither.  Cr uses Cb's type and its own offsets, and is filtered only when both types are >= 0
+// (sao.cpp:704-728).  Types outside -1..4 are off, bandPos is read & 31, offsets are any int8 (the result is clipped).
+// Transquant-bypass units (flags bit 2) then get the source samples back, whatever the SAO flags (origCUSampleRestoration).
+template <typename P>
+__global__ void __launch_bounds__(256) k_sao_apply_frame(const SaoApplyArgs a)
+{
+    __shared__ P s_t[66 * 66];
+    const int addr = blockIdx.x, p = blockIdx.y, tid = threadIdx.x;
+    if (p >= a.planes) return;
+    const int n = a.cols * a.rows;
+    const x265cu_sao_ctu prm = a.params[(size_t)p * n + addr];
+    int type = prm.typeIdx;
+    if (p == 2)
+    {
+        const int tcb = a.params[(size_t)n + addr].typeIdx;
+        type = type >= 0 && type <= 4 ? tcb : -1;
+    }
+    const bool sao = a.on[p] && type >= 0 && type <= 4;
+    if (!sao && !a.units) return;
+    const SaoCtuGeom g = sao_ctu_geom(a.width, a.height, a.log2Ctu, a.cols, addr, p);
+    const int log2S = a.log2Ctu - (p ? 1 : 0), S = 1 << log2S, T = g.w + 2;
+    P* plane = (P*)a.plane[p];
+    const ptrdiff_t st = p ? a.cstride : a.stride;
+    if (sao)
+    {
+        const P* lines = (const P*)a.lines[p];
+        const long rowLines = (long)a.rows * 2 * g.picW;
+        const int r = addr / a.cols, c = addr % a.cols;
+        for (int i = tid; i < T * (g.h + 2); i += blockDim.x)
+        {
+            const int tx = i % T, ty = i / T, px = g.lpelx + tx - 1, py = g.tpely + ty - 1;
+            P v = 0;
+            if (px >= 0 && px < g.picW && py >= 0 && py < g.picH)
+            {
+                if (ty == 0)               v = lines[((long)(r - 1) * 2 + 1) * g.picW + px];      // bottom row of the row above
+                else if (ty == g.h + 1)    v = lines[((long)(r + 1) * 2) * g.picW + px];          // top row of the row below
+                else if (tx == 0)          v = lines[rowLines + ((long)(c - 1) * 2 + 1) * g.picH + py];   // right column, left CTU
+                else if (tx == g.w + 1)    v = lines[rowLines + ((long)(c + 1) * 2) * g.picH + py];       // left column, right CTU
+                else                       v = plane[(ptrdiff_t)py * st + px];
+            }
+            s_t[ty * T + tx] = v;
+        }
+        __syncthreads();
+    }
+    const int x0 = type != 4 && type != 1 ? g.left : 0, x1 = type != 4 && type != 1 && g.right ? g.w - 1 : g.w;
+    const int y0 = type != 4 && type != 0 ? g.top : 0, y1 = type != 4 && type != 0 && g.bottom ? g.h - 1 : g.h;
+    const int dxa = type == 1 ? 0 : type == 3 ? 1 : -1, dya = type == 0 ? 0 : -1;   // neighbour a; b is the mirror
+    const int bandPos = prm.bandPos & 31, o0 = prm.offset[0], o1 = prm.offset[1], o2 = prm.offset[2], o3 = prm.offset[3];
+    const P* fenc = (const P*)a.fenc[p];
+    const ptrdiff_t fs = p ? a.fcstride : a.fstride;
+    const int us = p ? 1 : 2, upr = a.width >> 2;
+    for (int i = tid; i < S * S; i += blockDim.x)
+    {
+        const int x = i & (S - 1), y = i >> log2S;
+        if (x >= g.w || y >= g.h) continue;
+        const int px = g.lpelx + x, py = g.tpely + y;
+        if (a.units && (a.units[(size_t)(py >> us) * upr + (px >> us)].flags & 4))
+        {
+            plane[(ptrdiff_t)py * st + px] = fenc[(ptrdiff_t)py * fs + px];
+            continue;
+        }
+        if (!sao || x < x0 || x >= x1 || y < y0 || y >= y1) continue;
+        const P* t = s_t + (y + 1) * T + x + 1;
+        const int cv = t[0];
+        int o;
+        if (type == 4)
+        {
+            const int k = (sao_band<P>(cv) - bandPos) & 31;
+            o = k == 0 ? o0 : k == 1 ? o1 : k == 2 ? o2 : k == 3 ? o3 : 0;
+        }
+        else
+        {
+            const int et = sao_edge_type(cv, t[dya * T + dxa], t[-dya * T - dxa]);
+            o = et == 0 ? o0 : et == 1 ? o1 : et == 3 ? o2 : et == 4 ? o3 : 0;
+        }
+        plane[(ptrdiff_t)py * st + px] = (P)clipP<P>(cv + o);
+    }
+}
+
+// The calls' launches (arguments validated by the callers)
+template <typename P>
+static int launch_sao_stats_frame(x265cu_ctx* c, const SaoStatsArgs& a, int numCtus)
+{
+    k_sao_stats_frame<P><<<dim3(numCtus, 3), 256, 0, c->stream>>>(a);
+    CU_LAUNCH_CHECK(c);
+    return 0;
+}
+
+template <typename P>
+static int launch_sao_apply_frame(x265cu_ctx* c, SaoApplyArgs a)
+{
+    size_t need = 0, off[3] = { 0, 0, 0 };
+    for (int p = 0; p < a.planes; p++)
+    {
+        const int s = p ? 1 : 0;
+        off[p] = need;
+        if (a.on[p])
+            need += ((size_t)a.rows * 2 * (a.width >> s) + (size_t)a.cols * 2 * (a.height >> s)) * sizeof(P);
+        need = (need + 255) & ~(size_t)255;
+    }
+    if (need)
+    {
+        if (c->sao_lines_bytes < need)
+        {
+            if (c->d_sao_lines) { CU_CHECK(cudaStreamSynchronize(c->stream)); cudaFree(c->d_sao_lines); c->d_sao_lines = NULL; c->sao_lines_bytes = 0; }
+            CU_CHECK(cudaMalloc(&c->d_sao_lines, need));
+            c->sao_lines_bytes = need;
+        }
+        for (int p = 0; p < a.planes; p++) a.lines[p] = (uint8_t*)c->d_sao_lines + off[p];
+        k_sao_save_lines<P><<<dim3(2 * c->sm_count, 3), 256, 0, c->stream>>>(a);
+        CU_LAUNCH_CHECK(c);
+    }
+    if (need || a.units)
+    {
+        k_sao_apply_frame<P><<<dim3(a.cols * a.rows, 3), 256, 0, c->stream>>>(a);
+        CU_LAUNCH_CHECK(c);
+    }
+    return 0;
+}
+
 } // namespace lf

@@ -37,7 +37,7 @@ int x265cu_device_count(void)
 static void ctx_release(x265cu_ctx* c)
 {
     if (c->h_stage) cudaFreeHost(c->h_stage);
-    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state);
+    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state); cudaFree(c->d_sao_lines);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     for (int i = 0; i < 4; i++) if (c->me_ev[i]) cudaEventDestroy(c->me_ev[i]);
@@ -428,4 +428,75 @@ extern "C" int x265cu_deblock_frame(x265cu_ctx* c, int depth, void* luma, int st
     a.sliceType = p->sliceType; a.betaOffset = p->betaOffsetDiv2 * 2; a.tcOffset = p->tcOffsetDiv2 * 2;
     a.cbQpOffset = p->cbQpOffset; a.crQpOffset = p->crQpOffset; a.bypass = p->transquantBypass;
     return depth == 8 ? lf::launch_deblock_frame<uint8_t>(c, a) : lf::launch_deblock_frame<uint16_t>(c, a);
+}
+
+static_assert(sizeof(x265cu_sao_ctu) == 8, "SAO record (include/x265_b200.h)");
+
+// the argument rules both SAO calls share; NULL when they hold
+static const char* sao_check(const char* fn, int depth, int width, int height, int ctuSize, const void* y, const void* cb,
+                             const void* cr, int stride, int cstride)
+{
+    static char msg[160];
+    const char* why = NULL;
+    if (depth != 8 && depth != 10) why = "depth must be 8 or 10";
+    else if (width <= 0 || height <= 0 || (width & 7) || (height & 7)) why = "width and height must be positive multiples of 8";
+    else if (ctuSize != 16 && ctuSize != 32 && ctuSize != 64) why = "ctuSize must be 16, 32 or 64";
+    else if (!y) why = "NULL luma plane";
+    else if ((cb != NULL) != (cr != NULL)) why = "give both chroma planes or neither";
+    else if (stride < width || (cb && cstride < width / 2)) why = "stride smaller than the row";
+    if (!why) return NULL;
+    snprintf(msg, sizeof(msg), "%s: %s", fn, why);
+    return msg;
+}
+
+static int ilog2_ctu(int ctuSize) { return ctuSize == 64 ? 6 : ctuSize == 32 ? 5 : 4; }
+
+extern "C" int x265cu_sao_stats_frame(x265cu_ctx* c, int depth, int width, int height, int ctuSize,
+                                      const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                                      const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats)
+{
+    cudaSetDevice(c->device);
+    const char* fn = "x265cu_sao_stats_frame";
+    const char* bad = sao_check(fn, depth, width, height, ctuSize, rec_y, rec_cb, rec_cr, stride, cstride);
+    if (!bad) bad = sao_check(fn, depth, width, height, ctuSize, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
+    if (!bad && (fenc_cb != NULL) != (rec_cb != NULL)) bad = "x265cu_sao_stats_frame: give chroma for both the source and the reconstruction, or for neither";
+    if (!bad && !stats) bad = "x265cu_sao_stats_frame: NULL stats";
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    lf::SaoStatsArgs a;
+    a.fenc[0] = fenc_y; a.fenc[1] = fenc_cb; a.fenc[2] = fenc_cr;
+    a.rec[0] = rec_y; a.rec[1] = rec_cb; a.rec[2] = rec_cr;
+    a.fstride = fstride; a.fcstride = fcstride; a.stride = stride; a.cstride = cstride;
+    a.width = width; a.height = height; a.log2Ctu = ilog2_ctu(ctuSize);
+    a.cols = (width + ctuSize - 1) / ctuSize; a.planes = rec_cb ? 3 : 1; a.stats = stats;
+    const int n = a.cols * ((height + ctuSize - 1) / ctuSize);
+    return depth == 8 ? lf::launch_sao_stats_frame<uint8_t>(c, a, n) : lf::launch_sao_stats_frame<uint16_t>(c, a, n);
+}
+
+extern "C" int x265cu_sao_apply_frame(x265cu_ctx* c, int depth, int width, int height, int ctuSize,
+                                      void* y, void* cb, void* cr, int stride, int cstride,
+                                      const x265cu_sao_ctu* params, int saoLuma, int saoChroma, const x265cu_deblock_unit* units,
+                                      const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride)
+{
+    cudaSetDevice(c->device);
+    const char* fn = "x265cu_sao_apply_frame";
+    const char* bad = sao_check(fn, depth, width, height, ctuSize, y, cb, cr, stride, cstride);
+    if (!bad && !params) bad = "x265cu_sao_apply_frame: NULL parameters";
+    if (!bad && (saoLuma != 0 && saoLuma != 1 || saoChroma != 0 && saoChroma != 1)) bad = "x265cu_sao_apply_frame: saoLuma / saoChroma must be 0 or 1";
+    if (!bad && saoChroma && !cb) bad = "x265cu_sao_apply_frame: saoChroma set without chroma planes";
+    if (!bad && units)
+    {
+        bad = sao_check(fn, depth, width, height, ctuSize, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
+        if (!bad && (fenc_cb != NULL) != (cb != NULL)) bad = "x265cu_sao_apply_frame: bypass units need source planes for every plane filtered";
+    }
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    lf::SaoApplyArgs a;
+    a.plane[0] = y; a.plane[1] = cb; a.plane[2] = cr;
+    a.fenc[0] = fenc_y; a.fenc[1] = fenc_cb; a.fenc[2] = fenc_cr;
+    a.stride = stride; a.cstride = cstride; a.fstride = fstride; a.fcstride = fcstride;
+    a.width = width; a.height = height; a.log2Ctu = ilog2_ctu(ctuSize);
+    a.cols = (width + ctuSize - 1) / ctuSize; a.rows = (height + ctuSize - 1) / ctuSize; a.planes = cb ? 3 : 1;
+    a.on[0] = saoLuma; a.on[1] = a.on[2] = saoChroma;
+    a.params = params; a.units = units;
+    a.lines[0] = a.lines[1] = a.lines[2] = NULL;
+    return depth == 8 ? lf::launch_sao_apply_frame<uint8_t>(c, a) : lf::launch_sao_apply_frame<uint16_t>(c, a);
 }

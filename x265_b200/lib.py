@@ -42,6 +42,10 @@ DEBLOCK_UNIT = np.dtype([("qp", "i1"), ("flags", "u1"), ("log2CuSize", "u1"), ("
                          ("refPic", "i1", 2), ("mv", "<i2", (2, 2))], align=True)
 assert DEBLOCK_UNIT.itemsize == 16
 B_SLICE, P_SLICE, I_SLICE = 0, 1, 2
+# x265cu_sao_ctu: SaoCtuParam as the SAO decision leaves it; arrays [3][numCtus], CTU raster order
+SAO_CTU = np.dtype([("typeIdx", "i1"), ("bandPos", "u1"), ("offset", "i1", 4), ("pad", "u1", 2)])
+assert SAO_CTU.itemsize == 8
+SAO_STATS_PER_CTU = 2 * 3 * 5 * 32      # int32: [count, offsetOrg][plane][SaoType][class], two SAO::PerPlane
 
 
 class DeblockParams(C.Structure):
@@ -98,6 +102,8 @@ _PROTOS = {
     "x265cu_me_batch_chroma": (I, [P, I, P, I, P, I, P, P, I, P, I, P]),
     "x265cu_pred_cost_batch": (I, [P, I, P, I, P, I, P, P, I, P]),
     "x265cu_deblock_frame": (I, [P, I, P, I, P, P, I, I, I, P, P]),
+    "x265cu_sao_stats_frame": (I, [P, I, I, I, I, P, P, P, I, I, P, P, P, I, I, P]),
+    "x265cu_sao_apply_frame": (I, [P, I, I, I, I, P, P, P, I, I, P, I, I, P, P, P, P, I, I]),
 }
 
 
@@ -251,6 +257,24 @@ class Lib:
         uptr = units.ptr if isinstance(units, DeviceBuffer) else units
         self.check(self.L.x265cu_deblock_frame(self.ctx, depth, luma, stride, cb, cr, cstride, width, height, uptr, C.byref(params)))
 
+    def sao_stats_frame(self, depth, width, height, ctu, fenc, fstride, fcstride, rec, stride, cstride, stats):
+        """x265cu_sao_stats_frame: fenc / rec: (y, cb, cr) device addresses of pixel (0,0), cb = cr = None for luma only;
+        stats: device buffer (or address) of numCtus * SAO_STATS_PER_CTU int32."""
+        sptr = stats.ptr if isinstance(stats, DeviceBuffer) else stats
+        self.check(self.L.x265cu_sao_stats_frame(self.ctx, depth, width, height, ctu, fenc[0], fenc[1], fenc[2], fstride, fcstride,
+                                                 rec[0], rec[1], rec[2], stride, cstride, sptr))
+
+    def sao_apply_frame(self, depth, width, height, ctu, planes, stride, cstride, params, sao_luma, sao_chroma,
+                        bypass_units=None, fenc=(None, None, None), fstride=0, fcstride=0):
+        """x265cu_sao_apply_frame: applies the per-CTU SAO records (device buffer of [3][numCtus] SAO_CTU) to the planes (y,
+        cb, cr device addresses) in place; bypass_units: None or the DEBLOCK_UNIT map whose tq-bypass units get the
+        source samples (fenc) back."""
+        def addr(b):
+            return b.ptr if isinstance(b, DeviceBuffer) else b
+        self.check(self.L.x265cu_sao_apply_frame(self.ctx, depth, width, height, ctu, planes[0], planes[1], planes[2], stride, cstride,
+                                                 addr(params), sao_luma, sao_chroma, addr(bypass_units), fenc[0], fenc[1], fenc[2],
+                                                 fstride, fcstride))
+
     def mvcost_table(self, lam, rng):
         t = np.zeros(2 * rng + 1, np.uint16)
         self.L.x265cu_mvcost_table(C.c_double(lam), rng, t.ctypes.data)
@@ -314,6 +338,7 @@ _AN_PROTOS = {
     "x265cu_analyser_recon_to_ref_chroma": (I, [P, I, I, I, I]),
     "x265cu_analyser_ref_chroma_updated": (I, [P, I]),
     "x265cu_analyser_ref_plane_chroma": (P, [P, I, I, C.POINTER(I)]),
+    "x265cu_analyser_src_plane": (P, [P, I, C.POINTER(I)]),
 }
 STAGE_CHROMA_RESIDUAL = 8                 # analyser stage bit 3 (x265cu_analyser_enable_chroma_residual)
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
@@ -477,6 +502,14 @@ class Analyser:
         p = self.lib.L.x265cu_analyser_ref_plane_chroma(self.h, idx, plane, C.byref(st))
         if not p:
             raise RuntimeError("x265cu_analyser_ref_plane_chroma(%d, %d): no such plane (enable_chroma() first)" % (idx, plane))
+        return p, st.value
+
+    def src_plane(self, plane):
+        """(device address of pixel (0,0), stride in elements) of the resident source plane `plane` (0 luma, 1 Cb, 2 Cr)."""
+        st = I()
+        p = self.lib.L.x265cu_analyser_src_plane(self.h, plane, C.byref(st))
+        if not p:
+            raise RuntimeError("x265cu_analyser_src_plane(%d): no such plane (chroma: enable_chroma() first)" % plane)
         return p, st.value
 
     def h2d_bytes(self, field):
