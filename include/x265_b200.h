@@ -335,6 +335,23 @@ typedef struct {
 int x265cu_deblock_frame(x265cu_ctx*, int depth, void* luma_dev, int stride, void* cb_dev, void* cr_dev, int cstride,
                          int width, int height, const x265cu_deblock_unit* units_dev, const x265cu_deblock_params* params);
 
+/* ---------- the in-loop filters over a band of CTU rows [ctuRow0, ctuRow1) (row shards, row-by-row filtering) ----------
+ * Y0 = ctuRow0 * ctuSize and Y1 = min(height, ctuRow1 * ctuSize) are the band's luma rows, C0 = Y0 / 2 and C1 = Y1 / 2 its
+ * 4:2:0 chroma rows; every range below is clipped to the picture.  The arguments are those of the frame calls, with the
+ * same checks, plus ctuSize (16, 32 or 64; deblocking uses it only for the band's rows) and 0 <= ctuRow0 < ctuRow1 <=
+ * ceil(height / ctuSize); a call that breaks one returns -1 with x265cu_last_error() before any launch.  Records are read
+ * exactly as the frame calls read them.  Each band call is a pure function of the pre-deblock picture, so any partition of
+ * the CTU rows, on one plane or on separate per-GPU copies, in any order, gives the whole-picture result (INTEGRATION.md,
+ * "Row-range filtering"). */
+
+/* Writes dst luma rows [Y0-4, Y1+4) and chroma rows [C0-4, C1+4), full width, with the values x265cu_deblock_frame gives over
+ * the whole picture; reads src rows in the same ranges and unit rows [Y0/4-2, Y1/4+2).  src == dst (in place) is allowed
+ * when those src rows are still pre-deblock; otherwise the planes must not overlap. */
+int x265cu_deblock_rows(x265cu_ctx*, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                        const void* src_y, const void* src_cb, const void* src_cr, int sstride, int scstride,
+                        void* dst_y, void* dst_cb, void* dst_cr, int stride, int cstride,
+                        const x265cu_deblock_unit* units_dev, const x265cu_deblock_params* params);
+
 /* ---------- frame-level SAO (encoder/sao.cpp): statistics and apply; the decision stays on the host ----------
  * One slice per picture; 4:2:0, or 4:0:0 when every chroma pointer is NULL; CTU 16, 32 or 64.  Planes are device pointers at
  * pixel (0,0), strides in elements; both calls run on the context's stream.  Both read the deblocked, not-yet-SAO'd
@@ -359,6 +376,12 @@ typedef struct {
 int x265cu_sao_stats_frame(x265cu_ctx*, int depth, int width, int height, int ctuSize,
                            const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
                            const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats_dev);
+/* The records of the CTUs in rows [ctuRow0, ctuRow1) of the full-picture stats array; no other record is written.  Reads
+ * deblocked rows [Y0-1, Y1) / [C0-1, C1) (the statistics skip the bottom 4 luma / 2 chroma rows of a CTU above the picture
+ * bottom) and the same source rows. */
+int x265cu_sao_stats_rows(x265cu_ctx*, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                          const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                          const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats_dev);
 
 /* FrameFilter's processSaoCTU over every CTU (generateLumaOffsets / generateChromaOffsets / applyPixelOffsets, sao.cpp:274-732),
  * in place.  saoLuma / saoChroma: SAOParam::bSaoFlag[0 / 1].  Cr is filtered with Cb's type and its own offsets, and only
@@ -371,6 +394,14 @@ int x265cu_sao_apply_frame(x265cu_ctx*, int depth, int width, int height, int ct
                            const x265cu_sao_ctu* params_dev, int saoLuma, int saoChroma,
                            const x265cu_deblock_unit* bypass_units_dev,
                            const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride);
+/* Out of place: reads deblocked src rows [Y0-1, Y1+1) / [C0-1, C1+1); writes EVERY sample of dst rows [Y0, Y1) / [C0, C1)
+ * (filtered, copied where SAO is off, or restored from the source for bypass units) and nothing else.  Also returns -1 for
+ * src and dst planes that are the same. */
+int x265cu_sao_apply_rows(x265cu_ctx*, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                          const void* src_y, const void* src_cb, const void* src_cr, int sstride, int scstride,
+                          void* dst_y, void* dst_cb, void* dst_cr, int stride, int cstride,
+                          const x265cu_sao_ctu* params_dev, int saoLuma, int saoChroma, const x265cu_deblock_unit* bypass_units_dev,
+                          const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride);
 
 /* ---------- lookahead frame costs (BASELINE configs[1]; slicetype.cpp:696-805, 3115-3388) ----------
  * All pointers are device pointers.  Planes are the 4 lowres hpel planes of a frame (origin pixel,

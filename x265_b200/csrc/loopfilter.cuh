@@ -6,8 +6,8 @@
 // so all kernels read an unmodified input block and write a separate output block: one thread per sample, rows that pass
 // signs to the next row (E1 / E2 / E3 and the statistics) synchronise once per row.
 // Blocks are staged compactly by the per-call thunks (thunks.cuh); each kernel documents its layout.
-// The frame-level deblocking (k_deblock_frame, x265cu_deblock_frame) is the exception: it filters whole planes in place, since
-// the edges of one direction touch disjoint samples (see there).
+// The frame-level deblocking (k_deblock_frame, x265cu_deblock_frame / _rows) is the exception: it filters whole planes, or a
+// window of CTU rows, in place, since the edges of one direction touch disjoint samples (see there).
 #pragma once
 #include "common.cuh"
 
@@ -183,7 +183,23 @@ struct DeblockArgs
     int stride, cstride, width, height;
     const x265cu_deblock_unit* units;
     int sliceType, betaOffset, tcOffset, cbQpOffset, crQpOffset, bypass;   // offsets already doubled (deblock.cpp:328-329)
+    // The window (deblock_window): vertical pass over unit rows [s0, s1), filtering luma on [l0, l1) of them (the others
+    // only carry a chroma segment); horizontal pass over the edges [e0, e1) (luma y = 8e).
+    int s0, s1, l0, l1, e0, e1;
 };
+
+// The window of luma rows [y0, y1) (CTU-row aligned, y1 == height or a multiple of 16): the vertical pass covers unit rows
+// [y0/4 - 1, y1/4 + 1) in luma and the chroma segments of chroma rows [y0/2 - 4, y1/2 + 4), whose threads are the even unit
+// rows [y0/4 - 2, y1/4 + 2); the horizontal pass every edge y with y0 <= y <= y1 inside the picture.  Then luma rows
+// [y0 - 4, y1 + 4) and chroma rows [y0/2 - 4, y1/2 + 4) hold their whole-picture values and no other sample is written.
+// y0 = 0, y1 = height is the whole picture.
+__host__ __device__ inline void deblock_window(DeblockArgs& a, int y0, int y1)
+{
+    const int nu = a.height >> 2;
+    a.s0 = max(0, y0 / 4 - 2); a.s1 = min(nu, y1 / 4 + 2);
+    a.l0 = y0 / 4 - 1;         a.l1 = y1 / 4 + 1;
+    a.e0 = max(1, y0 / 8);     a.e1 = min(a.height >> 3, y1 / 8 + 1);
+}
 
 // Edge flag of the 8-sample edge at `pos` (x for vertical edges, y for horizontal ones) as Deblock::deblockCU leaves it at the Q
 // unit (deblock.cpp:90-93): the CU edge 2 (never the picture border: pos > 0 here), else a TU edge 2 (setEdgefilterTU), else an
@@ -232,13 +248,15 @@ __device__ __forceinline__ int boundary_strength(const x265cu_deblock_unit& p, c
 // touch disjoint samples: reads 4 / writes 3 per side, 2 / 1 for chroma).  DIR 0 (EDGE_VER): x = edge index e (luma x = 8e,
 // e >= 1), y = unit row a.  DIR 1 (EDGE_HOR): x = unit column a, y = edge index e (luma y = 8e).  The thread of an even e and
 // an even a also filters the chroma segment of that edge (4:2:0: chroma edges every 8 chroma samples, 4 chroma lines = the
-// 8 luma lines from unit a; deblock.cpp:104-113, 456-460).
-template <typename P, int DIR>
+// 8 luma lines from unit a; deblock.cpp:104-113, 456-460).  BAND: the launch covers the window of `a` (deblock_window);
+// otherwise the whole picture, and the window fields are not read (the frame call's code stays that of a whole-picture pass).
+template <typename P, int DIR, bool BAND>
 __global__ void __launch_bounds__(256) k_deblock_frame(const DeblockArgs a)
 {
     const int gx = blockIdx.x * blockDim.x + threadIdx.x, gy = blockIdx.y * blockDim.y + threadIdx.y;
-    const int e = (DIR == 0 ? gx : gy) + 1, s = DIR == 0 ? gy : gx;
-    if (DIR == 0 ? (e >= (a.width >> 3) || s >= (a.height >> 2)) : (e >= (a.height >> 3) || s >= (a.width >> 2))) return;
+    const int e = DIR == 0 ? gx + 1 : gy + (BAND ? a.e0 : 1), s = DIR == 0 ? gy + (BAND ? a.s0 : 0) : gx;
+    if (DIR == 0 ? (e >= (a.width >> 3) || s >= (BAND ? a.s1 : a.height >> 2))
+                 : (e >= (BAND ? a.e1 : a.height >> 3) || s >= (a.width >> 2))) return;
     const int upr = a.width >> 2;
     const size_t iq = DIR == 0 ? (size_t)s * upr + 2 * e : (size_t)(2 * e) * upr + s;
     const size_t ip = DIR == 0 ? iq - 1 : iq - upr;
@@ -256,7 +274,8 @@ __global__ void __launch_bounds__(256) k_deblock_frame(const DeblockArgs a)
     constexpr int shift = PixTraits<P>::depth - 8;
     const int qpA = ((int)up.qp + (int)uq.qp + 1) >> 1;
 
-    // luma (edgeFilterLuma, deblock.cpp:317-415)
+    // luma (edgeFilterLuma, deblock.cpp:317-415); a vertical-pass thread outside [l0, l1) only filters its chroma segment
+    if (DIR == 1 || !BAND || (s >= a.l0 && s < a.l1))
     {
         P* src = (P*)a.plane[0];
         const ptrdiff_t across = DIR == 0 ? 1 : a.stride, along = DIR == 0 ? a.stride : 1;
@@ -328,21 +347,26 @@ __global__ void __launch_bounds__(256) k_deblock_frame(const DeblockArgs a)
     }
 }
 
-// the two passes of x265cu_deblock_frame (arguments validated by the caller)
+// the two passes of x265cu_deblock_frame / x265cu_deblock_rows over the window in `a`; band: a window that is not the whole
+// picture (arguments validated by the caller)
 template <typename P>
-static int launch_deblock_frame(x265cu_ctx* c, const DeblockArgs& a)
+static int launch_deblock_frame(x265cu_ctx* c, const DeblockArgs& a, bool band)
 {
     const dim3 block(32, 8);
-    const int ne = (a.width >> 3) - 1, ns = a.height >> 2;             // vertical: edges x segments
-    if (ne > 0)
+    const int ne = (a.width >> 3) - 1, ns = a.s1 - a.s0;               // vertical: edges x segments
+    if (ne > 0 && ns > 0)
     {
-        k_deblock_frame<P, 0><<<dim3((ne + 31) / 32, (ns + 7) / 8), block, 0, c->stream>>>(a);
+        const dim3 grid((ne + 31) / 32, (ns + 7) / 8);
+        if (band) k_deblock_frame<P, 0, true><<<grid, block, 0, c->stream>>>(a);
+        else      k_deblock_frame<P, 0, false><<<grid, block, 0, c->stream>>>(a);
         CU_LAUNCH_CHECK(c);
     }
-    const int nh = (a.height >> 3) - 1, nc = a.width >> 2;             // horizontal: segments x edges
+    const int nh = a.e1 - a.e0, nc = a.width >> 2;                     // horizontal: segments x edges
     if (nh > 0)
     {
-        k_deblock_frame<P, 1><<<dim3((nc + 31) / 32, (nh + 7) / 8), block, 0, c->stream>>>(a);
+        const dim3 grid((nc + 31) / 32, (nh + 7) / 8);
+        if (band) k_deblock_frame<P, 1, true><<<grid, block, 0, c->stream>>>(a);
+        else      k_deblock_frame<P, 1, false><<<grid, block, 0, c->stream>>>(a);
         CU_LAUNCH_CHECK(c);
     }
     return 0;
@@ -511,10 +535,11 @@ struct SaoStatsArgs
 {
     const void* fenc[3]; const void* rec[3];   // at pixel (0,0); planes = 1: luma only
     int fstride, fcstride, stride, cstride, width, height, log2Ctu, cols, planes;
+    int row0;                                  // CTU row of blockIdx.x == 0: the grid covers CTU rows from row0 on
     int32_t* stats;                            // [numCtus][2][3][5][32]
 };
 
-// SAO::calcSaoStatsCTU (sao.cpp:735-917) of CTU blockIdx.x, plane blockIdx.y: every sample of the CTU once, classified for
+// SAO::calcSaoStatsCTU (sao.cpp:735-917) of CTU row0 * cols + blockIdx.x, plane blockIdx.y: every sample of the CTU once, classified for
 // each type inside that type's region (skipB 4 / skipR 5 away from the picture's right / bottom border, 2 / 3 in chroma; the
 // E0 rows ignore the picture bottom, sao.cpp:836).  Neighbour coordinates are clamped to the picture: the regions only hold
 // samples whose neighbours lie inside it.  Edge-type counts and sums stay in registers, band histograms in per-warp shared
@@ -525,7 +550,7 @@ __global__ void __launch_bounds__(256) k_sao_stats_frame(const SaoStatsArgs a)
     constexpr int NW = 8;
     __shared__ int s_bo[NW][2][32];
     __shared__ int s_eo[NW][2][4][5];
-    const int addr = blockIdx.x, p = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int addr = a.row0 * a.cols + blockIdx.x, p = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (int i = tid; i < NW * 2 * 32; i += blockDim.x) (&s_bo[0][0][0])[i] = 0;
     __syncthreads();
     int ec[4][5], es[4][5];
@@ -607,7 +632,9 @@ __global__ void __launch_bounds__(256) k_sao_stats_frame(const SaoStatsArgs a)
 struct SaoApplyArgs
 {
     void* plane[3]; const void* fenc[3];       // at pixel (0,0); planes = 1: luma only
-    int stride, cstride, fstride, fcstride, width, height, log2Ctu, cols, rows, planes;
+    const void* src[3];                        // the deblocked input: == plane (in place, through `lines`) or a separate plane
+    int stride, cstride, fstride, fcstride, sstride, scstride, width, height, log2Ctu, cols, rows, planes;
+    int row0;                                  // CTU row of blockIdx.x == 0: the grid covers CTU rows from row0 on
     int on[3];                                 // SAOParam::bSaoFlag per plane
     const x265cu_sao_ctu* params;              // [3][numCtus]
     const x265cu_deblock_unit* units;          // NULL: no transquant-bypass restoration
@@ -646,9 +673,10 @@ __global__ void __launch_bounds__(256) k_sao_save_lines(const SaoApplyArgs a)
     }
 }
 
-// processSaoCTU of CTU blockIdx.x, plane blockIdx.y (sao.cpp:274-732, framefilter.cpp:324-343), in place: the CTA stages its
-// CTU from the plane and a one-sample ring from the saved lines into shared memory, then writes the filtered samples of its
-// own CTU only.  Which samples a type changes: BO all; EO_0 not the picture's left / right column; EO_1 not its top /
+// processSaoCTU of CTU row0 * cols + blockIdx.x, plane blockIdx.y (sao.cpp:274-732, framefilter.cpp:324-343).  In place
+// (src == plane): the CTA stages its CTU from the plane and a one-sample ring from the saved lines into shared memory, then
+// writes the filtered samples of its own CTU only.  Out of place: it stages the CTU and the ring from src, which is never
+// written, and writes every sample of its CTU (filtered, else copied from src).  Which samples a type changes: BO all; EO_0 not the picture's left / right column; EO_1 not its top /
 // bottom row; EO_2 / EO_3 neither.  Cr uses Cb's type and its own offsets, and is filtered only when both types are >= 0
 // (sao.cpp:704-728).  Types outside -1..4 are off, bandPos is read & 31, offsets are any int8 (the result is clipped).
 // Transquant-bypass units (flags bit 2) then get the source samples back, whatever the SAO flags (origCUSampleRestoration).
@@ -656,7 +684,7 @@ template <typename P>
 __global__ void __launch_bounds__(256) k_sao_apply_frame(const SaoApplyArgs a)
 {
     __shared__ P s_t[66 * 66];
-    const int addr = blockIdx.x, p = blockIdx.y, tid = threadIdx.x;
+    const int addr = a.row0 * a.cols + blockIdx.x, p = blockIdx.y, tid = threadIdx.x;
     if (p >= a.planes) return;
     const int n = a.cols * a.rows;
     const x265cu_sao_ctu prm = a.params[(size_t)p * n + addr];
@@ -667,12 +695,23 @@ __global__ void __launch_bounds__(256) k_sao_apply_frame(const SaoApplyArgs a)
         type = type >= 0 && type <= 4 ? tcb : -1;
     }
     const bool sao = a.on[p] && type >= 0 && type <= 4;
-    if (!sao && !a.units) return;
+    const P* src = (const P*)(p == 0 ? a.src[0] : p == 1 ? a.src[1] : a.src[2]);
+    P* plane = (P*)(p == 0 ? a.plane[0] : p == 1 ? a.plane[1] : a.plane[2]);
+    const bool copy = src != plane;
+    if (!sao && !a.units && !copy) return;
     const SaoCtuGeom g = sao_ctu_geom(a.width, a.height, a.log2Ctu, a.cols, addr, p);
     const int log2S = a.log2Ctu - (p ? 1 : 0), S = 1 << log2S, T = g.w + 2;
-    P* plane = (P*)a.plane[p];
-    const ptrdiff_t st = p ? a.cstride : a.stride;
-    if (sao)
+    const ptrdiff_t st = p ? a.cstride : a.stride, sst = p ? a.scstride : a.sstride;
+    if (sao && copy)
+    {
+        for (int i = tid; i < T * (g.h + 2); i += blockDim.x)
+        {
+            const int tx = i % T, ty = i / T, px = g.lpelx + tx - 1, py = g.tpely + ty - 1;
+            s_t[ty * T + tx] = px >= 0 && px < g.picW && py >= 0 && py < g.picH ? src[(ptrdiff_t)py * sst + px] : (P)0;
+        }
+        __syncthreads();
+    }
+    else if (sao)
     {
         const P* lines = (const P*)a.lines[p];
         const long rowLines = (long)a.rows * 2 * g.picW;
@@ -710,7 +749,11 @@ __global__ void __launch_bounds__(256) k_sao_apply_frame(const SaoApplyArgs a)
             plane[(ptrdiff_t)py * st + px] = fenc[(ptrdiff_t)py * fs + px];
             continue;
         }
-        if (!sao || x < x0 || x >= x1 || y < y0 || y >= y1) continue;
+        if (!sao || x < x0 || x >= x1 || y < y0 || y >= y1)
+        {
+            if (copy) plane[(ptrdiff_t)py * st + px] = sao ? s_t[(y + 1) * T + x + 1] : src[(ptrdiff_t)py * sst + px];
+            continue;
+        }
         const P* t = s_t + (y + 1) * T + x + 1;
         const int cv = t[0];
         int o;
@@ -730,16 +773,25 @@ __global__ void __launch_bounds__(256) k_sao_apply_frame(const SaoApplyArgs a)
 
 // The calls' launches (arguments validated by the callers)
 template <typename P>
-static int launch_sao_stats_frame(x265cu_ctx* c, const SaoStatsArgs& a, int numCtus)
+static int launch_sao_stats_frame(x265cu_ctx* c, const SaoStatsArgs& a, int numCtus)     // CTUs from row a.row0 on
 {
     k_sao_stats_frame<P><<<dim3(numCtus, 3), 256, 0, c->stream>>>(a);
     CU_LAUNCH_CHECK(c);
     return 0;
 }
 
+// In place (src == plane): the line save, then the apply of every CTU.  Out of place: the apply of the CTU rows
+// [a.row0, row1) only, with no line save.
 template <typename P>
-static int launch_sao_apply_frame(x265cu_ctx* c, SaoApplyArgs a)
+static int launch_sao_apply_frame(x265cu_ctx* c, SaoApplyArgs a, int row1)
 {
+    const bool copy = a.src[0] != a.plane[0];
+    if (copy)
+    {
+        k_sao_apply_frame<P><<<dim3(a.cols * (row1 - a.row0), 3), 256, 0, c->stream>>>(a);
+        CU_LAUNCH_CHECK(c);
+        return 0;
+    }
     size_t need = 0, off[3] = { 0, 0, 0 };
     for (int p = 0; p < a.planes; p++)
     {

@@ -404,30 +404,91 @@ int x265cu_propagate_cost_batch(x265cu_ctx* c, int* dst, const uint16_t* propaga
 
 static_assert(sizeof(x265cu_deblock_unit) == 16 && sizeof(x265cu_deblock_params) == 24, "deblocking records (include/x265_b200.h)");
 
+// the argument rules of the deblocking calls on one set of planes; NULL when they hold
+static const char* deblock_check(const char* fn, int depth, int width, int height, const void* luma, const void* cb,
+                                 const void* cr, int stride, int cstride, const x265cu_deblock_unit* units,
+                                 const x265cu_deblock_params* p)
+{
+    static char msg[160];
+    const bool chroma = cb || cr;
+    const char* why = NULL;
+    if (depth != 8 && depth != 10) why = "depth must be 8 or 10";
+    else if (width <= 0 || height <= 0 || (width & 7) || (height & 7)) why = "width and height must be positive multiples of 8";
+    else if (!luma || !units || !p) why = "NULL luma plane, unit map or parameters";
+    else if (chroma && (!cb || !cr)) why = "give both chroma planes or neither";
+    else if (stride < width || (chroma && cstride < width / 2)) why = "stride smaller than the row";
+    else if (p->sliceType < 0 || p->sliceType > 2) why = "sliceType must be 0 (B), 1 (P) or 2 (I)";
+    else if (p->betaOffsetDiv2 < -6 || p->betaOffsetDiv2 > 6 || p->tcOffsetDiv2 < -6 || p->tcOffsetDiv2 > 6)
+        why = "beta / tc offsets (div 2) must be in -6..6";
+    else if (p->cbQpOffset < -12 || p->cbQpOffset > 12 || p->crQpOffset < -12 || p->crQpOffset > 12)
+        why = "chroma QP offsets must be in -12..12";
+    else if (p->transquantBypass != 0 && p->transquantBypass != 1) why = "transquantBypass must be 0 or 1";
+    if (!why) return NULL;
+    snprintf(msg, sizeof(msg), "%s: %s", fn, why);
+    return msg;
+}
+
+// the band rules the three row calls share; NULL when they hold
+static const char* rows_check(const char* fn, int height, int ctuSize, int ctuRow0, int ctuRow1)
+{
+    static char msg[160];
+    const char* why = NULL;
+    if (ctuSize != 16 && ctuSize != 32 && ctuSize != 64) why = "ctuSize must be 16, 32 or 64";
+    else if (ctuRow0 < 0 || ctuRow0 >= ctuRow1) why = "need 0 <= ctuRow0 < ctuRow1";
+    else if (height > 0 && ctuRow1 > (height + ctuSize - 1) / ctuSize) why = "ctuRow1 beyond the picture's last CTU row";
+    if (!why) return NULL;
+    snprintf(msg, sizeof(msg), "%s: %s", fn, why);
+    return msg;
+}
+
+static lf::DeblockArgs deblock_args(void* luma, void* cb, void* cr, int stride, int cstride, int width, int height,
+                                    const x265cu_deblock_unit* units, const x265cu_deblock_params* p, int y0, int y1)
+{
+    lf::DeblockArgs a;
+    a.plane[0] = luma; a.plane[1] = cb; a.plane[2] = cr;
+    a.stride = stride; a.cstride = cstride; a.width = width; a.height = height; a.units = units;
+    a.sliceType = p->sliceType; a.betaOffset = p->betaOffsetDiv2 * 2; a.tcOffset = p->tcOffsetDiv2 * 2;
+    a.cbQpOffset = p->cbQpOffset; a.crQpOffset = p->crQpOffset; a.bypass = p->transquantBypass;
+    lf::deblock_window(a, y0, y1);
+    return a;
+}
+
 extern "C" int x265cu_deblock_frame(x265cu_ctx* c, int depth, void* luma, int stride, void* cb, void* cr, int cstride,
                                     int width, int height, const x265cu_deblock_unit* units, const x265cu_deblock_params* p)
 {
     cudaSetDevice(c->device);
-    const bool chroma = cb || cr;
-    const char* bad = NULL;
-    if (depth != 8 && depth != 10) bad = "x265cu_deblock_frame: depth must be 8 or 10";
-    else if (width <= 0 || height <= 0 || (width & 7) || (height & 7)) bad = "x265cu_deblock_frame: width and height must be positive multiples of 8";
-    else if (!luma || !units || !p) bad = "x265cu_deblock_frame: NULL luma plane, unit map or parameters";
-    else if (chroma && (!cb || !cr)) bad = "x265cu_deblock_frame: give both chroma planes or neither";
-    else if (stride < width || (chroma && cstride < width / 2)) bad = "x265cu_deblock_frame: stride smaller than the row";
-    else if (p->sliceType < 0 || p->sliceType > 2) bad = "x265cu_deblock_frame: sliceType must be 0 (B), 1 (P) or 2 (I)";
-    else if (p->betaOffsetDiv2 < -6 || p->betaOffsetDiv2 > 6 || p->tcOffsetDiv2 < -6 || p->tcOffsetDiv2 > 6)
-        bad = "x265cu_deblock_frame: beta / tc offsets (div 2) must be in -6..6";
-    else if (p->cbQpOffset < -12 || p->cbQpOffset > 12 || p->crQpOffset < -12 || p->crQpOffset > 12)
-        bad = "x265cu_deblock_frame: chroma QP offsets must be in -12..12";
-    else if (p->transquantBypass != 0 && p->transquantBypass != 1) bad = "x265cu_deblock_frame: transquantBypass must be 0 or 1";
+    const char* bad = deblock_check("x265cu_deblock_frame", depth, width, height, luma, cb, cr, stride, cstride, units, p);
     if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
-    lf::DeblockArgs a;
-    a.plane[0] = luma; a.plane[1] = chroma ? cb : NULL; a.plane[2] = chroma ? cr : NULL;
-    a.stride = stride; a.cstride = cstride; a.width = width; a.height = height; a.units = units;
-    a.sliceType = p->sliceType; a.betaOffset = p->betaOffsetDiv2 * 2; a.tcOffset = p->tcOffsetDiv2 * 2;
-    a.cbQpOffset = p->cbQpOffset; a.crQpOffset = p->crQpOffset; a.bypass = p->transquantBypass;
-    return depth == 8 ? lf::launch_deblock_frame<uint8_t>(c, a) : lf::launch_deblock_frame<uint16_t>(c, a);
+    const lf::DeblockArgs a = deblock_args(luma, cb, cr, stride, cstride, width, height, units, p, 0, height);
+    return depth == 8 ? lf::launch_deblock_frame<uint8_t>(c, a, false) : lf::launch_deblock_frame<uint16_t>(c, a, false);
+}
+
+extern "C" int x265cu_deblock_rows(x265cu_ctx* c, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                                   const void* src_y, const void* src_cb, const void* src_cr, int sstride, int scstride,
+                                   void* dst_y, void* dst_cb, void* dst_cr, int stride, int cstride,
+                                   const x265cu_deblock_unit* units, const x265cu_deblock_params* p)
+{
+    cudaSetDevice(c->device);
+    const char* fn = "x265cu_deblock_rows";
+    const char* bad = deblock_check(fn, depth, width, height, dst_y, dst_cb, dst_cr, stride, cstride, units, p);
+    if (!bad) bad = deblock_check(fn, depth, width, height, src_y, src_cb, src_cr, sstride, scstride, units, p);
+    if (!bad && (src_cb != NULL) != (dst_cb != NULL)) bad = "x265cu_deblock_rows: give chroma for both the source and the destination, or for neither";
+    if (!bad) bad = rows_check(fn, height, ctuSize, ctuRow0, ctuRow1);
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    const int y0 = ctuRow0 * ctuSize, y1 = min(height, ctuRow1 * ctuSize), es = depth == 8 ? 1 : 2;
+    // out of place: the rows the passes read and write, luma [y0 - 4, y1 + 4) and chroma [y0/2 - 4, y1/2 + 4)
+    for (int k = 0; k < 3; k++)
+    {
+        const void* s = k == 0 ? src_y : k == 1 ? src_cb : src_cr;
+        void* d = k == 0 ? dst_y : k == 1 ? dst_cb : dst_cr;
+        if (!d || d == s) continue;
+        const int sh = k ? 1 : 0, r0 = max(0, (y0 >> sh) - 4), r1 = min(height >> sh, (y1 >> sh) + 4);
+        const size_t ss = (size_t)(k ? scstride : sstride) * es, ds = (size_t)(k ? cstride : stride) * es;
+        CU_CHECK(cudaMemcpy2DAsync((uint8_t*)d + r0 * ds, ds, (const uint8_t*)s + r0 * ss, ss, (size_t)(width >> sh) * es,
+                                   r1 - r0, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    const lf::DeblockArgs a = deblock_args(dst_y, dst_cb, dst_cr, stride, cstride, width, height, units, p, y0, y1);
+    return depth == 8 ? lf::launch_deblock_frame<uint8_t>(c, a, true) : lf::launch_deblock_frame<uint16_t>(c, a, true);
 }
 
 static_assert(sizeof(x265cu_sao_ctu) == 8, "SAO record (include/x265_b200.h)");
@@ -451,25 +512,87 @@ static const char* sao_check(const char* fn, int depth, int width, int height, i
 
 static int ilog2_ctu(int ctuSize) { return ctuSize == 64 ? 6 : ctuSize == 32 ? 5 : 4; }
 
-extern "C" int x265cu_sao_stats_frame(x265cu_ctx* c, int depth, int width, int height, int ctuSize,
-                                      const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
-                                      const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats)
+// x265cu_sao_stats_frame over CTU rows [ctuRow0, ctuRow1); fn names the call in the messages
+static int sao_stats(const char* fn, x265cu_ctx* c, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                     const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                     const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats)
 {
+    static char msg[200];
     cudaSetDevice(c->device);
-    const char* fn = "x265cu_sao_stats_frame";
     const char* bad = sao_check(fn, depth, width, height, ctuSize, rec_y, rec_cb, rec_cr, stride, cstride);
     if (!bad) bad = sao_check(fn, depth, width, height, ctuSize, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
-    if (!bad && (fenc_cb != NULL) != (rec_cb != NULL)) bad = "x265cu_sao_stats_frame: give chroma for both the source and the reconstruction, or for neither";
-    if (!bad && !stats) bad = "x265cu_sao_stats_frame: NULL stats";
+    if (!bad && (fenc_cb != NULL) != (rec_cb != NULL))
+        bad = (snprintf(msg, sizeof(msg), "%s: give chroma for both the source and the reconstruction, or for neither", fn), msg);
+    if (!bad && !stats) bad = (snprintf(msg, sizeof(msg), "%s: NULL stats", fn), msg);
+    if (!bad) bad = rows_check(fn, height, ctuSize, ctuRow0, ctuRow1);
     if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
     lf::SaoStatsArgs a;
     a.fenc[0] = fenc_y; a.fenc[1] = fenc_cb; a.fenc[2] = fenc_cr;
     a.rec[0] = rec_y; a.rec[1] = rec_cb; a.rec[2] = rec_cr;
     a.fstride = fstride; a.fcstride = fcstride; a.stride = stride; a.cstride = cstride;
     a.width = width; a.height = height; a.log2Ctu = ilog2_ctu(ctuSize);
-    a.cols = (width + ctuSize - 1) / ctuSize; a.planes = rec_cb ? 3 : 1; a.stats = stats;
-    const int n = a.cols * ((height + ctuSize - 1) / ctuSize);
+    a.cols = (width + ctuSize - 1) / ctuSize; a.planes = rec_cb ? 3 : 1; a.stats = stats; a.row0 = ctuRow0;
+    const int n = a.cols * (ctuRow1 - ctuRow0);
     return depth == 8 ? lf::launch_sao_stats_frame<uint8_t>(c, a, n) : lf::launch_sao_stats_frame<uint16_t>(c, a, n);
+}
+
+extern "C" int x265cu_sao_stats_frame(x265cu_ctx* c, int depth, int width, int height, int ctuSize,
+                                      const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                                      const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats)
+{
+    const int rows = ctuSize > 0 && height > 0 ? (height + ctuSize - 1) / ctuSize : 1;
+    return sao_stats("x265cu_sao_stats_frame", c, depth, width, height, ctuSize, 0, rows, fenc_y, fenc_cb, fenc_cr, fstride,
+                     fcstride, rec_y, rec_cb, rec_cr, stride, cstride, stats);
+}
+
+extern "C" int x265cu_sao_stats_rows(x265cu_ctx* c, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                                     const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride,
+                                     const void* rec_y, const void* rec_cb, const void* rec_cr, int stride, int cstride, int32_t* stats)
+{
+    return sao_stats("x265cu_sao_stats_rows", c, depth, width, height, ctuSize, ctuRow0, ctuRow1, fenc_y, fenc_cb, fenc_cr,
+                     fstride, fcstride, rec_y, rec_cb, rec_cr, stride, cstride, stats);
+}
+
+// x265cu_sao_apply_frame (src == dst, every CTU row) and x265cu_sao_apply_rows (src != dst, CTU rows [ctuRow0, ctuRow1))
+static int sao_apply(const char* fn, x265cu_ctx* c, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                     const void* sy, const void* scb, const void* scr, int sstride, int scstride,
+                     void* y, void* cb, void* cr, int stride, int cstride,
+                     const x265cu_sao_ctu* params, int saoLuma, int saoChroma, const x265cu_deblock_unit* units,
+                     const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride)
+{
+    static char msg[200];
+    cudaSetDevice(c->device);
+    const bool rows = sy != y;
+    const char* bad = sao_check(fn, depth, width, height, ctuSize, y, cb, cr, stride, cstride);
+    if (!bad && rows) bad = sao_check(fn, depth, width, height, ctuSize, sy, scb, scr, sstride, scstride);
+    if (!bad && rows && (scb != NULL) != (cb != NULL))
+        bad = (snprintf(msg, sizeof(msg), "%s: give chroma for both the source and the destination, or for neither", fn), msg);
+    if (!bad && rows && cb && (scb == cb || scr == cr))
+        bad = (snprintf(msg, sizeof(msg), "%s: the source and destination planes must differ", fn), msg);
+    if (!bad && !params) bad = (snprintf(msg, sizeof(msg), "%s: NULL parameters", fn), msg);
+    if (!bad && (saoLuma != 0 && saoLuma != 1 || saoChroma != 0 && saoChroma != 1))
+        bad = (snprintf(msg, sizeof(msg), "%s: saoLuma / saoChroma must be 0 or 1", fn), msg);
+    if (!bad && saoChroma && !cb) bad = (snprintf(msg, sizeof(msg), "%s: saoChroma set without chroma planes", fn), msg);
+    if (!bad && units)
+    {
+        bad = sao_check(fn, depth, width, height, ctuSize, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
+        if (!bad && (fenc_cb != NULL) != (cb != NULL))
+            bad = (snprintf(msg, sizeof(msg), "%s: bypass units need source planes for every plane filtered", fn), msg);
+    }
+    if (!bad) bad = rows_check(fn, height, ctuSize, ctuRow0, ctuRow1);
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    lf::SaoApplyArgs a;
+    a.plane[0] = y; a.plane[1] = cb; a.plane[2] = cr;
+    a.src[0] = sy; a.src[1] = scb; a.src[2] = scr;
+    a.fenc[0] = fenc_y; a.fenc[1] = fenc_cb; a.fenc[2] = fenc_cr;
+    a.stride = stride; a.cstride = cstride; a.sstride = sstride; a.scstride = scstride; a.fstride = fstride; a.fcstride = fcstride;
+    a.width = width; a.height = height; a.log2Ctu = ilog2_ctu(ctuSize);
+    a.cols = (width + ctuSize - 1) / ctuSize; a.rows = (height + ctuSize - 1) / ctuSize; a.planes = cb ? 3 : 1;
+    a.row0 = ctuRow0;
+    a.on[0] = saoLuma; a.on[1] = a.on[2] = saoChroma;
+    a.params = params; a.units = units;
+    a.lines[0] = a.lines[1] = a.lines[2] = NULL;
+    return depth == 8 ? lf::launch_sao_apply_frame<uint8_t>(c, a, ctuRow1) : lf::launch_sao_apply_frame<uint16_t>(c, a, ctuRow1);
 }
 
 extern "C" int x265cu_sao_apply_frame(x265cu_ctx* c, int depth, int width, int height, int ctuSize,
@@ -477,26 +600,23 @@ extern "C" int x265cu_sao_apply_frame(x265cu_ctx* c, int depth, int width, int h
                                       const x265cu_sao_ctu* params, int saoLuma, int saoChroma, const x265cu_deblock_unit* units,
                                       const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride)
 {
-    cudaSetDevice(c->device);
-    const char* fn = "x265cu_sao_apply_frame";
-    const char* bad = sao_check(fn, depth, width, height, ctuSize, y, cb, cr, stride, cstride);
-    if (!bad && !params) bad = "x265cu_sao_apply_frame: NULL parameters";
-    if (!bad && (saoLuma != 0 && saoLuma != 1 || saoChroma != 0 && saoChroma != 1)) bad = "x265cu_sao_apply_frame: saoLuma / saoChroma must be 0 or 1";
-    if (!bad && saoChroma && !cb) bad = "x265cu_sao_apply_frame: saoChroma set without chroma planes";
-    if (!bad && units)
+    const int rows = ctuSize > 0 && height > 0 ? (height + ctuSize - 1) / ctuSize : 1;
+    return sao_apply("x265cu_sao_apply_frame", c, depth, width, height, ctuSize, 0, rows, y, cb, cr, stride, cstride, y, cb, cr,
+                     stride, cstride, params, saoLuma, saoChroma, units, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
+}
+
+extern "C" int x265cu_sao_apply_rows(x265cu_ctx* c, int depth, int width, int height, int ctuSize, int ctuRow0, int ctuRow1,
+                                     const void* src_y, const void* src_cb, const void* src_cr, int sstride, int scstride,
+                                     void* dst_y, void* dst_cb, void* dst_cr, int stride, int cstride,
+                                     const x265cu_sao_ctu* params, int saoLuma, int saoChroma, const x265cu_deblock_unit* units,
+                                     const void* fenc_y, const void* fenc_cb, const void* fenc_cr, int fstride, int fcstride)
+{
+    if (src_y && src_y == dst_y)
     {
-        bad = sao_check(fn, depth, width, height, ctuSize, fenc_y, fenc_cb, fenc_cr, fstride, fcstride);
-        if (!bad && (fenc_cb != NULL) != (cb != NULL)) bad = "x265cu_sao_apply_frame: bypass units need source planes for every plane filtered";
+        x265cu_set_error("x265cu_sao_apply_rows: src_y == dst_y (the call is out of place)", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
     }
-    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
-    lf::SaoApplyArgs a;
-    a.plane[0] = y; a.plane[1] = cb; a.plane[2] = cr;
-    a.fenc[0] = fenc_y; a.fenc[1] = fenc_cb; a.fenc[2] = fenc_cr;
-    a.stride = stride; a.cstride = cstride; a.fstride = fstride; a.fcstride = fcstride;
-    a.width = width; a.height = height; a.log2Ctu = ilog2_ctu(ctuSize);
-    a.cols = (width + ctuSize - 1) / ctuSize; a.rows = (height + ctuSize - 1) / ctuSize; a.planes = cb ? 3 : 1;
-    a.on[0] = saoLuma; a.on[1] = a.on[2] = saoChroma;
-    a.params = params; a.units = units;
-    a.lines[0] = a.lines[1] = a.lines[2] = NULL;
-    return depth == 8 ? lf::launch_sao_apply_frame<uint8_t>(c, a) : lf::launch_sao_apply_frame<uint16_t>(c, a);
+    return sao_apply("x265cu_sao_apply_rows", c, depth, width, height, ctuSize, ctuRow0, ctuRow1, src_y, src_cb, src_cr, sstride,
+                     scstride, dst_y, dst_cb, dst_cr, stride, cstride, params, saoLuma, saoChroma, units, fenc_y, fenc_cb, fenc_cr,
+                     fstride, fcstride);
 }

@@ -104,6 +104,9 @@ _PROTOS = {
     "x265cu_deblock_frame": (I, [P, I, P, I, P, P, I, I, I, P, P]),
     "x265cu_sao_stats_frame": (I, [P, I, I, I, I, P, P, P, I, I, P, P, P, I, I, P]),
     "x265cu_sao_apply_frame": (I, [P, I, I, I, I, P, P, P, I, I, P, I, I, P, P, P, P, I, I]),
+    "x265cu_deblock_rows": (I, [P, I, I, I, I, I, I, P, P, P, I, I, P, P, P, I, I, P, P]),
+    "x265cu_sao_stats_rows": (I, [P, I, I, I, I, I, I, P, P, P, I, I, P, P, P, I, I, P]),
+    "x265cu_sao_apply_rows": (I, [P, I, I, I, I, I, I, P, P, P, I, I, P, P, P, I, I, P, I, I, P, P, P, P, I, I]),
 }
 
 
@@ -274,6 +277,29 @@ class Lib:
         self.check(self.L.x265cu_sao_apply_frame(self.ctx, depth, width, height, ctu, planes[0], planes[1], planes[2], stride, cstride,
                                                  addr(params), sao_luma, sao_chroma, addr(bypass_units), fenc[0], fenc[1], fenc[2],
                                                  fstride, fcstride))
+
+    # ---- the same filters over a band of CTU rows [r0, r1) (include/x265_b200.h, "the in-loop filters over a band") ----
+    def deblock_rows(self, depth, width, height, ctu, r0, r1, src, sstride, scstride, dst, stride, cstride, units, params):
+        """x265cu_deblock_rows: src / dst: (y, cb, cr) device addresses of pixel (0,0), cb = cr = None for luma only; writes dst
+        luma rows [Y0 - 4, Y1 + 4) and chroma rows [C0 - 4, C1 + 4) with the whole-picture deblocked values."""
+        uptr = units.ptr if isinstance(units, DeviceBuffer) else units
+        self.check(self.L.x265cu_deblock_rows(self.ctx, depth, width, height, ctu, r0, r1, src[0], src[1], src[2], sstride, scstride,
+                                              dst[0], dst[1], dst[2], stride, cstride, uptr, C.byref(params)))
+
+    def sao_stats_rows(self, depth, width, height, ctu, r0, r1, fenc, fstride, fcstride, rec, stride, cstride, stats):
+        """x265cu_sao_stats_rows: the records of the CTUs in rows [r0, r1) of the full-picture stats array."""
+        sptr = stats.ptr if isinstance(stats, DeviceBuffer) else stats
+        self.check(self.L.x265cu_sao_stats_rows(self.ctx, depth, width, height, ctu, r0, r1, fenc[0], fenc[1], fenc[2], fstride,
+                                                fcstride, rec[0], rec[1], rec[2], stride, cstride, sptr))
+
+    def sao_apply_rows(self, depth, width, height, ctu, r0, r1, src, sstride, scstride, dst, stride, cstride, params, sao_luma,
+                       sao_chroma, bypass_units=None, fenc=(None, None, None), fstride=0, fcstride=0):
+        """x265cu_sao_apply_rows: out of place, writes every sample of dst rows [Y0, Y1) / [C0, C1) from the deblocked src."""
+        def addr(b):
+            return b.ptr if isinstance(b, DeviceBuffer) else b
+        self.check(self.L.x265cu_sao_apply_rows(self.ctx, depth, width, height, ctu, r0, r1, src[0], src[1], src[2], sstride, scstride,
+                                                dst[0], dst[1], dst[2], stride, cstride, addr(params), sao_luma, sao_chroma,
+                                                addr(bypass_units), fenc[0], fenc[1], fenc[2], fstride, fcstride))
 
     def mvcost_table(self, lam, rng):
         t = np.zeros(2 * rng + 1, np.uint16)

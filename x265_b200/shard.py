@@ -77,3 +77,51 @@ def exchange_rows(dist, plane_tensor, nrows, world, height, stride, margin_y, es
     for w in works:
         w.wait()
     return plane_tensor
+
+
+# ---- in-loop filtering of row shards (include/x265_b200.h, x265cu_deblock_rows / _sao_stats_rows / _sao_apply_rows) ----
+# A band's deblocking reads and writes pre-deblock luma rows [Y0 - 4, Y1 + 4) and chroma rows [C0 - 4, C1 + 4), so before it
+# each rank needs only the 4 luma and 4 chroma rows on either side of its bands from the neighbours that own them; the
+# statistics and the apply then read only rows the rank's own deblocking wrote.  Per frame a row shard runs: run_rows,
+# exchange_halos of the reconstruction, deblock_rows (recon -> per-rank deblocked scratch), sao_stats_rows, the host's SAO
+# decision, sao_apply_rows (scratch -> the resident reference band), exchange_rows of the final bands, ref_updated.
+
+def filter_halo(r0, r1, ctu, height):
+    """((y0, y1), (c0, c1)): the luma and 4:2:0 chroma rows x265cu_deblock_rows reads (and writes) for CTU rows [r0, r1)."""
+    Y0, Y1 = r0 * ctu, min(height, r1 * ctu)
+    return (max(0, Y0 - 4), min(height, Y1 + 4)), (max(0, Y0 // 2 - 4), min(height // 2, Y1 // 2 + 4))
+
+
+def halo_sends(nrows, world, height, ctu, mode="block"):
+    """[(src_rank, (y0, y1), (c0, c1)), ...]: the pre-deblock luma / chroma rows each owner broadcasts so that every rank
+    holds the halos of its bands.  At every boundary between CTU rows of different owners, each side sends the 4 luma and 4
+    chroma rows next to it (a CTU row is at least 8 luma rows high, so they are the owner's own rows)."""
+    out = []
+    for r in range(1, nrows):
+        above, below = row_owner(r - 1, nrows, world, mode), row_owner(r, nrows, world, mode)
+        if above == below:
+            continue
+        y, c = r * ctu, r * ctu // 2
+        out.append((above, (y - 4, y), (c - 4, c)))
+        out.append((below, (y, min(height, y + 4)), (c, min(height // 2, c + 4))))
+    return out
+
+
+def exchange_halos(dist, luma, chroma, nrows, world, height, ctu, stride, cstride=0, margin_y=0, cmargin_y=0, es=1,
+                   mode="block"):
+    """Broadcast-only exchange of the pre-deblock halo rows (halo_sends) between the ranks of a row shard.  `luma`: flat
+    uint8 view of the whole luma plane allocation (row stride `stride` pixels, picture row 0 at allocation row `margin_y`);
+    `chroma`: () or the (cb, cr) allocations likewise with `cstride` / `cmargin_y`; `es` bytes per pixel.  Returns the
+    number of bytes broadcast."""
+    if world <= 1:
+        return 0
+    works, nbytes = [], 0
+    for src, (y0, y1), (c0, c1) in halo_sends(nrows, world, height, ctu, mode):
+        parts = [(luma, y0, y1, stride, margin_y)] + [(p, c0, c1, cstride, cmargin_y) for p in chroma]
+        for t, a, b, st, my in parts:
+            b0, b1 = (my + a) * st * es, (my + b) * st * es
+            works.append(dist.broadcast(t[b0:b1], src=src, async_op=True))
+            nbytes += b1 - b0
+    for w in works:
+        w.wait()
+    return nbytes
