@@ -428,6 +428,42 @@ int x265cu_lookahead_cost_batch(x265cu_ctx*, int depth, const x265cu_la_job* job
 int x265cu_propagate_cost_batch(x265cu_ctx*, int* dst_dev, const uint16_t* propagateIn_dev, const int32_t* intraCosts_dev,
                                 const uint16_t* interCosts_dev, const int32_t* invQscales_dev, double fpsFactor, int64_t len);
 
+/* cuTree's propagation chain: Lookahead::cuTree (slicetype.cpp:2538-2639) with every estimateCUPropagate step
+ * (:2641-2747) on the device, in stream order, without a host round trip.  What stays with the caller: the singleCost
+ * calls (the estimates must exist before the call; x265cu_cutree_estimates lists them) and cuTreeFinish, which the host
+ * runs, in the order of `finish`, on the propagateCost of the listed frames (its log2 is the host's libm).
+ *
+ * frames[0..numframes] are HOST records of device pointers, the reference's Lowres fields:
+ *   intraCost, invQscale    Lowres::intraCost / invQscaleFactor (invQscaleFactor8x8 when rc.qgSize == 8), per lowres CU
+ *   propagateCost           in / out (2-byte aligned); cleared, accumulated and swapped as the reference does: on return
+ *                           the pointers of frames[0] and frames[lastnonb] are exchanged where :2572 / :2633 exchange them
+ *   lowresCosts[d0][d1]     the estimate (b - d0, b + d1, b) of this frame (LOWRES_COST_SHIFT list bits); NULL: not supplied
+ *   mvs[list][dist]         Lowres::lowresMvs[list][dist] as int32 (x, y) pairs, the layout of x265cu_la_job
+ *   sliceType               X265_TYPE_* (only X265_TYPE_B = 5 against the rest matters)
+ * A P estimate (b == p1) must carry list-0 bits only, as every estimate of the lookahead does.
+ * finish (2 * maxFinish ints) receives (frame, ref0Distance) per cuTreeFinish call, in the reference's order (with VBV the
+ * in-chain calls of :2745-2746 first).  ref0Distance -1 marks the lookahead-less intra case (:2561-2571): the host copies
+ * qpAqOffset to qpCuTreeOffset instead.  Returns the number of finish entries, or -1 before any launch (x265cu_last_error)
+ * when an estimate or motion field the chain reads was not supplied, an invQscale / propagateCost pointer is NULL, or the
+ * window reaches the reference's estimateCUPropagate(0, 0, 0) (lookaheadDepth 0 without an anchor after frame 0). */
+#define X265CU_CUTREE_DIST 18                                /* X265_BFRAME_MAX + 2 */
+typedef struct {
+    const int32_t* intraCost; const int32_t* invQscale; uint16_t* propagateCost;
+    const uint16_t* lowresCosts[X265CU_CUTREE_DIST][X265CU_CUTREE_DIST];
+    const int32_t* mvs[2][X265CU_CUTREE_DIST];
+    int32_t sliceType, reserved;
+} x265cu_cutree_frame;
+typedef struct {
+    int32_t bIntra, lookaheadDepth, bBPyramid, bEnableWeightedBiPred, vbv;   /* vbv: rc.vbvBufferSize != 0 */
+    int32_t fpsNum, fpsDenom;
+} x265cu_cutree_params;
+int x265cu_cutree(x265cu_ctx*, x265cu_cutree_frame* frames, int numframes, const x265cu_cutree_params* params, int w8, int h8,
+                  int32_t* finish, int maxFinish);
+/* The (p0, p1, b) estimates x265cu_cutree reads for these slice types (sliceTypes[0..numframes]), in the order the
+ * reference's singleCost calls them: 3 ints each into triples (room for maxTriples).  Returns the count, or -1. */
+int x265cu_cutree_estimates(const int32_t* sliceTypes, int numframes, const x265cu_cutree_params* params, int32_t* triples,
+                            int maxTriples);
+
 /* Lookahead weighted-prediction analysis: LookaheadTLD::weightsAnalyse + weightCostLuma (slicetype.cpp:807-840, 860-961), the
  * call estimateFrameCost makes before the L0 search when --weightp is on (slicetype.cpp:3137).  Planes are whole padded
  * lowres buffers (Lowres::buffer[i], lowres.cpp:132-139: `planesize` pixels each, picture origin at `padoffset`), device

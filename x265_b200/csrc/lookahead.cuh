@@ -300,18 +300,125 @@ __device__ __forceinline__ int la_cvttsd2si(double v)
 {
     return (v >= -2147483648.0 && v < 2147483648.0) ? (int)v : (int)0x80000000;
 }
+// The amount of one CU: shared by k_propagate_cost and cuTree's step kernels (k_cutree_amount).
+__device__ __forceinline__ int la_propagate_amount(int propagateIn, int intraCost, int interCostWord, int invQscale, double fps)
+{
+    const int interCost = min(intraCost, interCostWord & LA_COST_MASK);
+    // Q16 x Q8.8 = Q24.8, an int32 product converted to double: it wraps past 2^31 as the reference's does
+    const double propagateIntra = (double)(int)((unsigned)intraCost * (unsigned)invQscale);
+    const double propagateAmount = __dadd_rn((double)propagateIn, __dmul_rn(propagateIntra, fps));
+    const double propagateNum = (double)(intraCost - interCost);
+    const double propagateDenom = (double)intraCost;
+    return la_cvttsd2si(__dadd_rn(__ddiv_rn(__dmul_rn(propagateAmount, propagateNum), propagateDenom), 0.5));
+}
 __global__ void __launch_bounds__(256) k_propagate_cost(int* __restrict__ dst, const uint16_t* __restrict__ propagateIn, const int32_t* __restrict__ intraCosts,
                                                         const uint16_t* __restrict__ interCosts, const int32_t* __restrict__ invQscales, double fpsFactor, int64_t len)
 {
     const double fps = fpsFactor / 256;                             // range [0.01, 1.00]
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += (int64_t)gridDim.x * blockDim.x)
+        dst[i] = la_propagate_amount(propagateIn[i], intraCosts[i], interCosts[i], invQscales[i], fps);
+}
+
+// ---------------------------------------------------------------------------------------------
+// cuTree's propagation chain (Lookahead::cuTree / estimateCUPropagate, slicetype.cpp:2538-2747).  x265cu_cutree groups the
+// window's steps into levels: steps of which none reads an array that another one writes (the non-referenced B steps of a
+// mini-GOP; then the middle B of a b-pyramid; then the anchor).  A level is two launches in stream order:
+//   k_cutree_amount  : every CU's propagate_amount into scratch, and the level's overflow flag;
+//   k_cutree_scatter : the bipred weighting, the MV-0 shortcut, the bilinear split and the edge tests of :2690-2738.
+// Why the parallel scatter is exact: every add is CLIP_ADD(s, x) = (uint16)min(s + x, 65535).  For x >= 0 the result of
+// any sequence of such adds on one word is min(s0 + sum(x), 65535) whatever their order (each add is monotone and the clamp
+// absorbs), so the adds of a whole level may land in any order -- as a compare-and-swap loop on the 16-bit word that
+// applies min(s + x, 65535) atomically.  x >= 0 holds when every propagating amount is below 2^21: then
+// amount * bipredWeight + 32 (weights <= 64) and listamount * idxNweight + 512 (weights <= 1024) stay inside int32.  The
+// reference computes those products in int32 and wraps (x86 imul): a wrapped add can be negative, CLIP_ADD then wraps
+// modulo 2^16 and the result depends on the order.  k_cutree_amount raises the flag for any amount >= 2^21; the scatter
+// then replays the whole level on one thread, in the reference's step and raster order, with its int32 wrap-around.
+#define CUTREE_MAX_STEPS 16
+#define CUTREE_SAFE_AMOUNT (1 << 21)
+struct CuTreeStep
+{
+    const int32_t* intraCost; const int32_t* invQscale;
+    const uint16_t* propagateIn;        // frame b's own propagateCost when referenced, NULL: zeros (:2656-2658)
+    const uint16_t* lowresCosts;        // lowresCosts[b - p0][p1 - b]
+    const int32_t* mvs[2];              // lowresMvs[list][listDist[list]] as int32 pairs
+    uint16_t* ref[2];                   // propagateCost of p0 and p1
+    int32_t bipredWeight[2];
+};
+struct CuTreeLevel
+{
+    CuTreeStep s[CUTREE_MAX_STEPS];
+    int n;
+};
+
+__global__ void __launch_bounds__(256) k_cutree_amount(const CuTreeLevel L, int ncu, double fpsFactor, int* __restrict__ amounts, int* __restrict__ flag)
+{
+    const CuTreeStep& s = L.s[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ncu) return;
+    const int amount = la_propagate_amount(s.propagateIn ? s.propagateIn[i] : 0, s.intraCost[i], s.lowresCosts[i], s.invQscale[i], fpsFactor / 256);
+    amounts[blockIdx.y * ncu + i] = amount;
+    if (amount >= CUTREE_SAFE_AMOUNT) *flag = 1;
+}
+
+// CLIP_ADD(s, x) exactly as the compiled reference computes it: int32 sum (wrapping), min with 65535, truncation to 16 bits
+__device__ __forceinline__ void cutree_clip_add_serial(uint16_t* p, int x)
+{
+    *p = (uint16_t)min((int)((unsigned)*p + (unsigned)x), 65535);
+}
+// the same for 0 <= x < 2^31 - 65535, atomically: min(s + x, 65535) on the 16-bit word
+__device__ __forceinline__ void cutree_clip_add_atomic(uint16_t* p, int x)
+{
+    if (x <= 0) return;
+    unsigned short old = *(volatile unsigned short*)p, assumed;
+    do
     {
-        const int intraCost = intraCosts[i];
-        const int interCost = min(intraCost, (int)(interCosts[i] & LA_COST_MASK));
-        const double propagateIntra = __dmul_rn((double)intraCost, (double)invQscales[i]);              // Q16 x Q8.8 = Q24.8
-        const double propagateAmount = __dadd_rn((double)propagateIn[i], __dmul_rn(propagateIntra, fps));
-        const double propagateNum = (double)(intraCost - interCost);
-        const double propagateDenom = (double)intraCost;
-        dst[i] = la_cvttsd2si(__dadd_rn(__ddiv_rn(__dmul_rn(propagateAmount, propagateNum), propagateDenom), 0.5));
+        assumed = old;
+        if (assumed == 0xffff) return;
+        old = atomicCAS((unsigned short*)p, assumed, (unsigned short)min((int)assumed + x, 65535));
+    } while (old != assumed);
+}
+
+// One CU of one step (:2676-2741); products in unsigned arithmetic so that they wrap as the reference's int32 ones do
+template <bool Serial>
+__device__ __forceinline__ void cutree_scatter_cu(const CuTreeStep& s, int cu, int amount, int w8, int h8)
+{
+    if (amount <= 0) return;                                          // intra blocks do not propagate
+    const int listsUsed = s.lowresCosts[cu] >> LA_COST_SHIFT;
+    const int blocky = cu / w8, blockx = cu - blocky * w8;
+    auto add = [&](uint16_t* p, int x) { if (Serial) cutree_clip_add_serial(p, x); else cutree_clip_add_atomic(p, x); };
+    auto part = [](int a, int w) { return (int)((unsigned)a * (unsigned)w + 512u) >> 10; };
+    for (int list = 0; list < 2; list++)
+    {
+        if (!((listsUsed >> list) & 1)) continue;
+        int listamount = amount;
+        if (listsUsed == 3) listamount = (int)((unsigned)listamount * (unsigned)s.bipredWeight[list] + 32u) >> 6;
+        uint16_t* ref = s.ref[list];
+        const int mx = s.mvs[list][2 * cu], my = s.mvs[list][2 * cu + 1];
+        if (!(mx | my)) { add(ref + cu, listamount); continue; }     // the MV-0 shortcut
+        const int cux = (mx >> 5) + blockx, cuy = (my >> 5) + blocky;
+        const int idx0 = cux + cuy * w8, x = mx & 31, y = my & 31;
+        const int w0 = (32 - y) * (32 - x), w1 = (32 - y) * x, w2 = y * (32 - x), w3 = y * x;
+        const bool x0 = cux >= 0 && cux < w8, x1 = cux + 1 >= 0 && cux + 1 < w8;
+        const bool y0 = cuy >= 0 && cuy < h8, y1 = cuy + 1 >= 0 && cuy + 1 < h8;
+        if (x0 && y0) add(ref + idx0, part(listamount, w0));
+        if (x1 && y0) add(ref + idx0 + 1, part(listamount, w1));
+        if (x0 && y1) add(ref + idx0 + w8, part(listamount, w2));
+        if (x1 && y1) add(ref + idx0 + w8 + 1, part(listamount, w3));
     }
+}
+
+__global__ void __launch_bounds__(256) k_cutree_scatter(const CuTreeLevel L, int w8, int h8, const int* __restrict__ amounts, const int* __restrict__ flag)
+{
+    const int ncu = w8 * h8;
+    if (*flag)
+    {
+        // an amount of the level may overflow: the whole level on one thread, in the reference's order
+        if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0)
+            for (int k = 0; k < L.n; k++)
+                for (int cu = 0; cu < ncu; cu++)
+                    cutree_scatter_cu<true>(L.s[k], cu, amounts[k * ncu + cu], w8, h8);
+        return;
+    }
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < ncu) cutree_scatter_cu<false>(L.s[blockIdx.y], i, amounts[blockIdx.y * ncu + i], w8, h8);
 }

@@ -14,6 +14,8 @@
 #include "lookahead.cuh"
 #include <math.h>
 #include <mutex>
+#include <vector>
+#include <algorithm>
 
 static thread_local char g_err[512] = "";
 unsigned long long g_x265cu_launches = 0;
@@ -37,7 +39,7 @@ int x265cu_device_count(void)
 static void ctx_release(x265cu_ctx* c)
 {
     if (c->h_stage) cudaFreeHost(c->h_stage);
-    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state); cudaFree(c->d_sao_lines);
+    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state); cudaFree(c->d_sao_lines); cudaFree(c->d_cutree);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     for (int i = 0; i < 4; i++) if (c->me_ev[i]) cudaEventDestroy(c->me_ev[i]);
@@ -619,4 +621,275 @@ extern "C" int x265cu_sao_apply_rows(x265cu_ctx* c, int depth, int width, int he
     return sao_apply("x265cu_sao_apply_rows", c, depth, width, height, ctuSize, ctuRow0, ctuRow1, src_y, src_cb, src_cr, sstride,
                      scstride, dst_y, dst_cb, dst_cr, stride, cstride, params, saoLuma, saoChroma, units, fenc_y, fenc_cb, fenc_cr,
                      fstride, fcstride);
+}
+
+// ---------------------------------------------------------------------------------------------
+// cuTree's propagation chain (Lookahead::cuTree, slicetype.cpp:2538-2639) on the device
+namespace {
+enum { CT_EST, CT_CLEAR, CT_STEP, CT_SWAP, CT_FINISH, CT_COPY_AQ };
+struct CtOp { int kind, a, b, c, d; };
+const int CT_TYPE_B = 5;                                              // X265_TYPE_B
+
+// The reference's control flow as a list of operations: the singleCost calls (CT_EST p0 p1 b), the memsets, the steps
+// (CT_STEP p0 p1 b referenced), the pointer swaps and the cuTreeFinish calls (CT_FINISH frame ref0Distance).
+const char* cutree_plan(const int32_t* st, int numframes, const x265cu_cutree_params* p, std::vector<CtOp>& ops)
+{
+    const int idx = !p->bIntra;
+    int lastnonb, curnonb = 1, bframes = 0;
+    int i = numframes;
+    while (i > 0 && st[i] == CT_TYPE_B)
+        i--;
+    lastnonb = i;
+    auto op = [&](int k, int a, int b = 0, int c = 0, int d = 0) { ops.push_back(CtOp{ k, a, b, c, d }); };
+    auto step = [&](int p0, int p1, int b, int referenced) {
+        op(CT_STEP, p0, p1, b, referenced);
+        if (p->vbv && p->lookaheadDepth && referenced)
+            op(CT_FINISH, b, b == p1 ? b - p0 : 0);                   // :2745-2746
+    };
+    if (!p->lookaheadDepth)
+    {
+        if (p->bIntra)
+        {
+            op(CT_CLEAR, 0);
+            op(CT_COPY_AQ, 0);
+            return NULL;
+        }
+        op(CT_SWAP, lastnonb, 0);
+        op(CT_CLEAR, 0);
+    }
+    else
+    {
+        if (lastnonb < idx)
+            return NULL;
+        op(CT_CLEAR, lastnonb);
+    }
+    while (i-- > idx)
+    {
+        curnonb = i;
+        while (st[curnonb] == CT_TYPE_B && curnonb > 0)
+            curnonb--;
+        if (curnonb < idx)
+            break;
+        op(CT_EST, curnonb, lastnonb, lastnonb);
+        op(CT_CLEAR, curnonb);
+        bframes = lastnonb - curnonb - 1;
+        if (p->bBPyramid && bframes > 1)
+        {
+            const int middle = (bframes + 1) / 2 + curnonb;
+            op(CT_EST, curnonb, lastnonb, middle);
+            op(CT_CLEAR, middle);
+            while (i > curnonb)
+            {
+                const int p0 = i > middle ? middle : curnonb;
+                const int p1 = i < middle ? middle : lastnonb;
+                if (i != middle)
+                {
+                    op(CT_EST, p0, p1, i);
+                    step(p0, p1, i, 0);
+                }
+                i--;
+            }
+            step(curnonb, lastnonb, middle, 1);
+        }
+        else
+        {
+            while (i > curnonb)
+            {
+                op(CT_EST, curnonb, lastnonb, i);
+                step(curnonb, lastnonb, i, 0);
+                i--;
+            }
+        }
+        step(curnonb, lastnonb, lastnonb, 1);
+        lastnonb = curnonb;
+    }
+    if (!p->lookaheadDepth)
+    {
+        if (lastnonb == 0)
+            return "the window reaches estimateCUPropagate(0, 0, 0) (lookaheadDepth 0 without an anchor after frame 0)";
+        op(CT_EST, 0, lastnonb, lastnonb);
+        step(0, lastnonb, lastnonb, 1);
+        op(CT_SWAP, lastnonb, 0);
+    }
+    op(CT_FINISH, lastnonb, lastnonb);
+    if (p->bBPyramid && bframes > 1 && !p->vbv)
+        op(CT_FINISH, lastnonb + (bframes + 1) / 2, 0);
+    for (const CtOp& o : ops)
+        if (o.kind == CT_EST && (o.c - o.a >= X265CU_CUTREE_DIST || o.b - o.c >= X265CU_CUTREE_DIST))
+            return "a mini-GOP is longer than X265_BFRAME_MAX + 1 frames";
+    return NULL;
+}
+
+const char* cutree_args(const int32_t* st, int numframes, const x265cu_cutree_params* p, std::vector<CtOp>& ops)
+{
+    if (!st || !p || numframes < 0)
+        return "NULL frames / parameters or numframes < 0";
+    if (p->fpsNum <= 0 || p->fpsDenom <= 0)
+        return "fpsNum and fpsDenom must be positive";
+    return cutree_plan(st, numframes, p, ops);
+}
+
+double clip_duration(double f) { return std::min(std::max(0.01, f), 1.00); }   // CLIP_DURATION (ratecontrol.h:42-47)
+} // namespace
+
+extern "C" int x265cu_cutree_estimates(const int32_t* sliceTypes, int numframes, const x265cu_cutree_params* params, int32_t* triples,
+                                       int maxTriples)
+{
+    std::vector<CtOp> ops;
+    const char* bad = cutree_args(sliceTypes, numframes, params, ops);
+    int n = 0;
+    for (const CtOp& o : ops)
+        if (o.kind == CT_EST)
+        {
+            if (n >= maxTriples || !triples) { bad = "more estimates than maxTriples"; break; }
+            triples[3 * n] = o.a; triples[3 * n + 1] = o.b; triples[3 * n + 2] = o.c;
+            n++;
+        }
+    if (bad)
+    {
+        static thread_local char msg[256];
+        snprintf(msg, sizeof(msg), "x265cu_cutree_estimates: %s", bad);
+        x265cu_set_error(msg, cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    return n;
+}
+
+extern "C" int x265cu_cutree(x265cu_ctx* c, x265cu_cutree_frame* frames, int numframes, const x265cu_cutree_params* p, int w8, int h8,
+                             int32_t* finish, int maxFinish)
+{
+    static thread_local char msg[256];
+    cudaSetDevice(c->device);
+    std::vector<CtOp> ops;
+    std::vector<int32_t> st(numframes >= 0 && frames ? numframes + 1 : 0);
+    for (size_t f = 0; f < st.size(); f++)
+        st[f] = frames[f].sliceType;
+    const char* bad = frames ? cutree_args(st.data(), numframes, p, ops) : "NULL frames";
+    if (!bad && (w8 <= 0 || h8 <= 0))
+        bad = "w8 and h8 must be positive";
+    int nfinish = 0, nsteps = 0;
+    for (size_t k = 0; k < ops.size() && !bad; k++)
+    {
+        const CtOp& o = ops[k];
+        if (o.kind == CT_FINISH || o.kind == CT_COPY_AQ)
+            nfinish++;
+        if (o.kind == CT_CLEAR && !frames[o.a].propagateCost)
+            bad = (snprintf(msg, sizeof(msg), "frame %d: NULL propagateCost", o.a), msg);
+        if (o.kind != CT_STEP)
+            continue;
+        nsteps++;
+        const int p0 = o.a, p1 = o.b, b = o.c;
+        const x265cu_cutree_frame& f = frames[b];
+        if (!frames[p0].propagateCost || !frames[p1].propagateCost || !f.propagateCost)
+            bad = (snprintf(msg, sizeof(msg), "step (%d, %d, %d): NULL propagateCost", p0, p1, b), msg);
+        else if (!f.intraCost || !f.invQscale)
+            bad = (snprintf(msg, sizeof(msg), "frame %d: NULL intraCost or invQscale", b), msg);
+        else if (!f.lowresCosts[b - p0][p1 - b])
+            bad = (snprintf(msg, sizeof(msg), "estimate (%d, %d, %d) not supplied (lowresCosts[%d][%d])", p0, p1, b, b - p0, p1 - b), msg);
+        else if (!f.mvs[0][b - p0] || (p1 > b && !f.mvs[1][p1 - b]))
+            bad = (snprintf(msg, sizeof(msg), "estimate (%d, %d, %d): motion field not supplied", p0, p1, b), msg);
+    }
+    if (!bad && nfinish > maxFinish)
+        bad = (snprintf(msg, sizeof(msg), "%d cuTreeFinish calls, room for %d", nfinish, maxFinish), msg);
+    if (!bad && nfinish && !finish)
+        bad = "NULL finish list";
+    const int ncu = w8 * h8;
+    const size_t amountBytes = (size_t)CUTREE_MAX_STEPS * ncu * 4, need = amountBytes + (size_t)(nsteps + 1) * 4;
+    if (!bad && c->cutree_bytes < need)
+    {
+        cudaFree(c->d_cutree);
+        c->d_cutree = NULL; c->cutree_bytes = 0;
+        if (cudaMalloc(&c->d_cutree, need) != cudaSuccess) { x265cu_set_error("x265cu_cutree: scratch", cudaGetLastError(), __FILE__, __LINE__); return -1; }
+        c->cutree_bytes = need;
+    }
+    if (bad)
+    {
+        static thread_local char full[320];
+        snprintf(full, sizeof(full), "x265cu_cutree: %s", bad);
+        x265cu_set_error(full, cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    int* amounts = (int*)c->d_cutree;
+    int* flags = (int*)((char*)c->d_cutree + amountBytes);
+    CU_CHECK(cudaMemsetAsync(flags, 0, (size_t)(nsteps + 1) * 4, c->stream));
+
+    double totalDuration = 0.0;                                       // :2545-2549, the summing loop
+    for (int j = 0; j <= numframes; j++)
+        totalDuration += (double)p->fpsDenom / p->fpsNum;
+    const double averageDuration = totalDuration / (numframes + 1);
+    const double fpsFactor = clip_duration((double)p->fpsDenom / p->fpsNum) / clip_duration(averageDuration);   // :2654
+
+    std::vector<uint16_t*> pc(numframes + 1);
+    for (int f = 0; f <= numframes; f++)
+        pc[f] = frames[f].propagateCost;
+    // the pending level: its steps and the arrays they read (their own propagateCost) and add into (p0's, p1's)
+    CuTreeLevel L;
+    L.n = 0;
+    std::vector<const uint16_t*> R, W;
+    int level = 0;
+    auto has = [](const std::vector<const uint16_t*>& v, const uint16_t* q) { return std::find(v.begin(), v.end(), q) != v.end(); };
+    auto flush = [&]() -> int {
+        if (!L.n) return 0;
+        const dim3 grid((ncu + 255) / 256, L.n);
+        int* flag = flags + level++;
+        k_cutree_amount<<<grid, 256, 0, c->stream>>>(L, ncu, fpsFactor, amounts, flag);
+        CU_LAUNCH_CHECK(c);
+        k_cutree_scatter<<<grid, 256, 0, c->stream>>>(L, w8, h8, amounts, flag);
+        CU_LAUNCH_CHECK(c);
+        L.n = 0; R.clear(); W.clear();
+        return 0;
+    };
+    // a memset runs at once in stream order, after the launched levels and before the pending one: legal when the pending
+    // level does not touch the array (the reference's memset precedes every pending step that touches it)
+    auto zero = [&](uint16_t* q, size_t n) -> int {
+        if ((has(R, q) || has(W, q)) && flush()) return -1;
+        CU_CHECK(cudaMemsetAsync(q, 0, n * sizeof(uint16_t), c->stream));
+        return 0;
+    };
+    nfinish = 0;
+    for (const CtOp& o : ops)
+    {
+        switch (o.kind)
+        {
+        case CT_CLEAR:
+            if (zero(pc[o.a], ncu)) return -1;
+            break;
+        case CT_SWAP:
+            std::swap(pc[o.a], pc[o.b]);
+            break;
+        case CT_FINISH:
+        case CT_COPY_AQ:
+            finish[2 * nfinish] = o.a; finish[2 * nfinish + 1] = o.kind == CT_FINISH ? o.b : -1;
+            nfinish++;
+            break;
+        case CT_STEP:
+        {
+            const int p0 = o.a, p1 = o.b, b = o.c, referenced = o.d;
+            if (!referenced && zero(pc[b], w8)) return -1;            // :2657-2658, row 0 of b's own array
+            const uint16_t* in = referenced ? pc[b] : NULL;
+            if (L.n == CUTREE_MAX_STEPS || (in && has(W, in)) || has(R, pc[p0]) || (p1 > b && has(R, pc[p1])))
+                if (flush()) return -1;
+            const x265cu_cutree_frame& f = frames[b];
+            CuTreeStep& s = L.s[L.n++];
+            s.intraCost = f.intraCost; s.invQscale = f.invQscale; s.propagateIn = in;
+            s.lowresCosts = f.lowresCosts[b - p0][p1 - b];
+            s.mvs[0] = f.mvs[0][b - p0];
+            s.mvs[1] = p1 > b ? f.mvs[1][p1 - b] : f.mvs[0][b - p0];  // a P estimate has no list-1 CUs
+            s.ref[0] = pc[p0]; s.ref[1] = pc[p1];
+            const int distScaleFactor = (((b - p0) << 8) + ((p1 - p0) >> 1)) / (p1 - p0);
+            const int bipredWeight = p->bEnableWeightedBiPred ? 64 - (distScaleFactor >> 2) : 32;
+            s.bipredWeight[0] = bipredWeight; s.bipredWeight[1] = 64 - bipredWeight;
+            if (in) R.push_back(in);
+            W.push_back(pc[p0]);
+            if (p1 > b) W.push_back(pc[p1]);
+            break;
+        }
+        default:
+            break;
+        }
+    }
+    if (flush()) return -1;
+    for (int f = 0; f <= numframes; f++)
+        frames[f].propagateCost = pc[f];
+    return nfinish;
 }

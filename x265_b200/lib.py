@@ -325,6 +325,22 @@ LA_JOB = np.dtype([("fenc", "<u8", 4), ("ref0", "<u8", 4), ("ref1", "<u8", 4), (
 assert LA_INTRA_JOB.itemsize == 56 and LA_JOB.itemsize == 184
 
 
+# ---------------- cuTree's propagation chain (x265cu_cutree) ----------------
+CUTREE_DIST = 18                          # X265CU_CUTREE_DIST = X265_BFRAME_MAX + 2
+TYPE_I, TYPE_P, TYPE_B = 2, 3, 5          # X265_TYPE_* (x265.h)
+
+
+class CutreeFrame(C.Structure):
+    """x265cu_cutree_frame: device pointers of one frame's cuTree inputs (include/x265_b200.h)."""
+    _fields_ = [("intraCost", P), ("invQscale", P), ("propagateCost", P), ("lowresCosts", P * CUTREE_DIST * CUTREE_DIST),
+                ("mvs", P * CUTREE_DIST * 2), ("sliceType", C.c_int32), ("reserved", C.c_int32)]
+
+
+class CutreeParams(C.Structure):
+    _fields_ = [("bIntra", C.c_int32), ("lookaheadDepth", C.c_int32), ("bBPyramid", C.c_int32), ("bEnableWeightedBiPred", C.c_int32),
+                ("vbv", C.c_int32), ("fpsNum", C.c_int32), ("fpsDenom", C.c_int32)]
+
+
 # ---------------- frame-level analyser (x265cu_analyser_*) ----------------
 class AnalysisParams(C.Structure):
     _fields_ = [("width", I), ("height", I), ("depth", I), ("numRefs", I), ("method", I), ("subme", I), ("merange", I),
@@ -371,6 +387,8 @@ _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I
 _AN_PROTOS["x265cu_lowres_intra_batch"] = (I, [P, I, P, I, I, I, I, I])
 _AN_PROTOS["x265cu_lookahead_cost_batch"] = (I, [P, I, P, I, I, I, I, P])
 _AN_PROTOS["x265cu_lookahead_weights_analyse"] = (I, [P, I, P, P, P, I64, I, I, I, I64, P, P, P])
+_AN_PROTOS["x265cu_cutree"] = (I, [P, P, I, P, I, I, P, I])
+_AN_PROTOS["x265cu_cutree_estimates"] = (I, [P, I, P, P, I])
 _PROTOS.update(_AN_PROTOS)
 
 

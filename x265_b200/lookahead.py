@@ -71,8 +71,11 @@ class _PlaneView:
 class Lookahead:
     """Device-resident lookahead window of `nframes` frames of one geometry."""
 
-    def __init__(self, lib, W, H, depth, nframes, lookahead_slices=0):
+    def __init__(self, lib, W, H, depth, nframes, lookahead_slices=0, keep_costs=False):
+        """keep_costs: keep every estimate's per-CU lowresCosts resident on the device (Lowres::lowresCosts[b - p0][p1 - b]),
+        as cu_tree() needs them; by default they live in a recycled per-launch block."""
         self.cu, self.depth, self.W, self.H, self.n = lib, depth, W, H, nframes
+        self.keep_costs = keep_costs
         self.nslices, self.rows_per_slice = coop_slices(H, lookahead_slices)
         self.w8, self.h8, self.ls = lowres_geometry(W, H)
         self.ncu = self.w8 * self.h8
@@ -86,7 +89,7 @@ class Lookahead:
             lib.check(lib.L.x265cu_memset(lib.ctx, block.ptr, 0, block.nbytes))
             planes = [_PlaneView(block, k * self.plane_bytes, self.plane_bytes) for k in range(4)]
             self.fr.append(dict(block=block, planes=planes, intraCost=lib.alloc(4 * self.ncu), intraMode=lib.alloc(self.ncu),
-                                lc0=lib.alloc(2 * self.ncu), rs0=lib.alloc(4 * self.h8), out0=lib.alloc(16), mvs={}, mvcosts={}, res={},
+                                lc0=lib.alloc(2 * self.ncu), rs0=lib.alloc(4 * self.h8), out0=lib.alloc(16), mvs={}, mvcosts={}, res={}, lc={}, prop=None,
                                 has_planes=False, has_intra=False, invq=None))
         self.tab = lib.to_device(lib.mvcost_table(LOOKAHEAD_LAMBDA[depth], MVRANGE))
         self._full = None
@@ -174,7 +177,7 @@ class Lookahead:
         bufs = []
         # the batch's results land in three blocks (per-CU costs, row sums, frame totals): one D2H each in collect_batch()
         nt = len(todo)
-        lcB = self._take(2 * self.ncu * nt) if nt else None
+        lcB = self._take(2 * self.ncu * nt) if nt and not self.keep_costs else None
         rsB = self._take(4 * self.h8 * nt) if nt else None
         outB = self._take(32 * nt) if nt else None
         for ti, (p0, p1, b) in enumerate(todo):
@@ -195,7 +198,11 @@ class Lookahead:
                     cu.check(cu.L.x265cu_memset(cu.ctx, f["mvcosts"][(lst, dist)].ptr, 0, 4 * self.ncu))
                 j["doSearch%d" % lst] = int(new and (lst == 0 or p1 > b))
                 j["mvs"][lst] = f["mvs"][(lst, dist)].ptr; j["mvcosts"][lst] = f["mvcosts"][(lst, dist)].ptr
-            lc = _PlaneView(lcB, ti * 2 * self.ncu, 2 * self.ncu); rs = _PlaneView(rsB, ti * 4 * self.h8, 4 * self.h8); out = _PlaneView(outB, ti * 32, 24)
+            if self.keep_costs:
+                lc = f["lc"][(d0, d1)] = self._take(2 * self.ncu)
+            else:
+                lc = _PlaneView(lcB, ti * 2 * self.ncu, 2 * self.ncu)
+            rs = _PlaneView(rsB, ti * 4 * self.h8, 4 * self.h8); out = _PlaneView(outB, ti * 32, 24)
             bufs.append((lc, rs, out))
             j["intraCost"] = f["intraCost"].ptr; j["invQscale"] = f["invq"].ptr if f["invq"] is not None else 0; j["lowresCosts"] = lc.ptr; j["rowSatds"] = rs.ptr; j["out"] = out.ptr
             # cooperative slices (slicetype.cpp:3143): one job per slice, each an independent wavefront over its CU rows
@@ -227,7 +234,10 @@ class Lookahead:
         nt = len(prep["todo"])
         if nt:
             outs = outB.download(np.int64, 4 * nt).reshape(nt, 4)
-            lcs = lcB.download(np.uint16, self.ncu * nt).reshape(nt, self.ncu) if full else None
+            lcs = None
+            if full:
+                lcs = np.stack([lc.download(np.uint16, self.ncu) for lc, _, _ in prep["bufs"]]) if self.keep_costs else \
+                    lcB.download(np.uint16, self.ncu * nt).reshape(nt, self.ncu)
             rss = rsB.download(np.int32, self.h8 * nt).reshape(nt, self.h8) if full else None
         for ti, (p0, p1, b) in enumerate(prep["todo"]):
             o = outs[ti]
@@ -252,7 +262,7 @@ class Lookahead:
     def forget_results(self):
         """Drop cached estimates and motion fields (bench: re-run the same window)."""
         for f in self.fr:
-            for d in (f["mvs"], f["mvcosts"]):
+            for d in (f["mvs"], f["mvcosts"], f["lc"]):
                 for v in d.values():
                     self._give(v)
                 d.clear()
@@ -265,6 +275,8 @@ class Lookahead:
                 f[k].free()
             if f["invq"] is not None:
                 f["invq"].free()
+            if f["prop"] is not None:
+                f["prop"].free()
         self.tab.free()
         if self._full is not None:
             self._full.free()
@@ -272,6 +284,66 @@ class Lookahead:
             for b in free:
                 b.free()
         self._pool.clear()
+
+
+    # ---- cuTree: Lookahead::cuTree's propagation chain on the device (x265cu_cutree) ----
+    def cu_tree(self, slice_types, b_intra=False, lookahead_depth=40, b_pyramid=True, weighted_bipred=False, vbv=False, fps=(25, 1),
+                world=1, rank=0):
+        """Lookahead::cuTree (slicetype.cpp:2538-2639) over frames 0..len(slice_types)-1 of the window, up to cuTreeFinish.
+        Computes the estimates the chain reads that are not resident yet (cost_batch, in conflict-free launches), runs the
+        chain on the device and downloads only the propagateCost of the frames cuTreeFinish is then called on.
+        Returns (finish, costs): finish = [(frame, ref0Distance)] in the reference's order (-1: the lookahead-less intra case,
+        qpAqOffset copied), costs = {frame: propagateCost (uint16 per lowres CU)}.  Needs keep_costs=True and every frame's
+        invQscale (set_invqscale: invQscaleFactor, or invQscaleFactor8x8 when rc.qgSize == 8).  With frame shards
+        (world > 1) every estimate must live on this rank: cuTree across ranks is not supported."""
+        from .lib import CutreeFrame, CutreeParams
+        import ctypes as C
+        cu = self.cu
+        if not self.keep_costs:
+            raise ValueError("cu_tree needs the estimates' lowresCosts resident: construct Lookahead with keep_costs=True")
+        numframes = len(slice_types) - 1
+        if numframes < 0 or numframes >= self.n:
+            raise ValueError("cu_tree: %d frames, the window holds %d" % (numframes + 1, self.n))
+        prm = CutreeParams(int(b_intra), lookahead_depth, int(b_pyramid), int(weighted_bipred), int(vbv), fps[0], fps[1])
+        st = np.ascontiguousarray(slice_types, np.int32)
+        cap = 4 * (numframes + 2) * 18
+        tri = np.zeros(3 * cap, np.int32)
+        n = cu.L.x265cu_cutree_estimates(st.ctypes.data, numframes, C.byref(prm), tri.ctypes.data, cap)
+        if n < 0:
+            raise RuntimeError(cu.last_error())
+        triples = [tuple(int(v) for v in tri[3 * k:3 * k + 3]) for k in range(n)]
+        for (p0, p1, b) in triples:
+            if owner(b, world) != rank:
+                raise ValueError("cu_tree: estimate (%d, %d, %d) lives on rank %d, not on rank %d; cuTree across lookahead frame "
+                                 "shards is not supported" % (p0, p1, b, owner(b, world), rank))
+        missing = [t for t in dict.fromkeys(triples) if (t[2] - t[0], t[1] - t[2]) not in self.fr[t[2]]["res"]]
+        for batch in conflict_free_batches(missing):
+            self.cost_batch(batch, full=False)
+        recs = (CutreeFrame * (numframes + 1))()
+        byptr = {}
+        for i in range(numframes + 1):
+            f = self.fr[i]
+            if f["prop"] is None:
+                f["prop"] = cu.alloc(2 * self.ncu)
+            byptr[f["prop"].ptr] = f["prop"]
+            r = recs[i]
+            r.intraCost = f["intraCost"].ptr
+            r.invQscale = f["invq"].ptr if f["invq"] is not None else None
+            r.propagateCost = f["prop"].ptr
+            r.sliceType = int(st[i])
+            for (d0, d1), lc in f["lc"].items():
+                r.lowresCosts[d0][d1] = lc.ptr
+            for (lst, dist), mv in f["mvs"].items():
+                r.mvs[lst][dist] = mv.ptr
+        fin = np.zeros(2 * (numframes + 2), np.int32)
+        nf = cu.L.x265cu_cutree(cu.ctx, recs, numframes, C.byref(prm), self.w8, self.h8, fin.ctypes.data, numframes + 2)
+        if nf < 0:
+            raise RuntimeError(cu.last_error())
+        for i in range(numframes + 1):                 # the reference's propagateCost pointer swaps
+            self.fr[i]["prop"] = byptr[recs[i].propagateCost]
+        finish = [(int(fin[2 * k]), int(fin[2 * k + 1])) for k in range(nf)]
+        costs = {f: self.fr[f]["prop"].download(np.uint16, self.ncu) for f, d in finish if d >= 0}
+        return finish, costs
 
 
 def window_triples(nframes, bframes):
