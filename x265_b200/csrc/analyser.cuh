@@ -31,6 +31,8 @@ struct x265cu_analyser
     // first PU job / CU / TU of every CTU row (+ one past the end): the lists are in CTU raster order, so a CTU-row
     // range [r0, r1) is one contiguous slice of each list (what a WPP row shard owns, frameencoder.cpp:850-868)
     int ctuRows; std::vector<int> rowJob, rowCu, rowTu;
+    // per-size TU and CU lists of the residual and intra launches and their CTU-row offsets (geometry.h tuBy / cuBy)
+    int32_t* d_tuBy[3]; int32_t* d_cuBy[4]; std::vector<int> rowTuBy[3], rowCuBy[4];
     // 4:2:0 chroma planes for the chroma-SATD term of subpelCompare (x265cu_analyser_enable_chroma): half resolution,
     // stride / 2 elements per row, margins = half the luma margins (picyuv.cpp:87-94)
     int chromaOn, cstride, cRows; size_t cPlaneBytes, cOrgBytes;
@@ -72,6 +74,8 @@ static void an_build_geometry(x265cu_analyser* a)
     a->ctuRows = g.ctuRows; a->rowJob.swap(g.rowJob); a->rowCu.swap(g.rowCu); a->rowTu.swap(g.rowTu);
     a->njobs = (int)a->pus.size(); a->ncu = (int)a->cus.size(); a->ntu = (int)a->tus.size(); a->ncoef = g.ncoef;
     a->d_order = an_upload(a->ctx, g.order);
+    for (int k = 0; k < 3; k++) { a->d_tuBy[k] = an_upload(a->ctx, g.tuBy[k]); a->rowTuBy[k].swap(g.rowTuBy[k]); }
+    for (int k = 0; k < 4; k++) { a->d_cuBy[k] = an_upload(a->ctx, g.cuBy[k]); a->rowCuBy[k].swap(g.rowCuBy[k]); }
     for (int k = 0; k < 3; k++)
     {
         std::vector<MeGroup> grp(g.grpFirst[k].size());
@@ -185,8 +189,9 @@ static bool an_chroma_reach_ok(const x265cu_analyser* a, int r0, int r1)
     return geometry_chroma_reach_inside(u, a->p.width, a->p.height, a->cstride, AN_MARGIN_X / 2, AN_MARGIN_Y / 2);
 }
 
-// the residual stage of the luma plane or of both 4:2:0 chroma planes over the CUs [cu0, cu0 + ncu) and their TUs
-static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int tu0, int ntu)
+// the residual stage of the luma plane or of both 4:2:0 chroma planes over the CUs [cu0, cu0 + ncu) and their TUs, the
+// CTU rows [r0, r1)
+static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int r0, int r1)
 {
     x265cu_ctx* c = a->ctx;
     const int npl = chroma ? 2 : 1;
@@ -199,12 +204,14 @@ static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int tu
         r.qp[p] = chroma ? a->qpC[p] : a->p.qp;
     }
     r.stride = chroma ? a->cstride : a->stride; r.recon = chroma ? a->d_reconCTable : a->d_reconTable;
-    r.cus = a->d_cus; r.tus = a->d_tus + tu0; r.ntu = ntu; r.cu_jobs = a->d_cu_jobs; r.numRefs = a->p.numRefs; r.me_out = a->d_me_out;
+    r.cus = a->d_cus; r.tus = a->d_tus; r.cu_jobs = a->d_cu_jobs; r.numRefs = a->p.numRefs; r.me_out = a->d_me_out;
     r.cu_sse = chroma ? a->d_cu_sseC : a->d_cu_sse; r.cu_numsig = chroma ? a->d_cu_numsigC : a->d_cu_numsig;
     r.cu_ref = chroma ? NULL : a->d_cu_ref;
     CU_CHECK(cudaMemsetAsync(r.cu_sse + (size_t)npl * cu0, 0, sizeof(unsigned long long) * npl * ncu, c->stream));
     CU_CHECK(cudaMemsetAsync(r.cu_numsig + (size_t)npl * cu0, 0, sizeof(uint32_t) * npl * ncu, c->stream));
-    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r) : launch_resid<uint16_t>(c, chroma, r);
+    const int32_t* lists[3]; int n[3];
+    for (int k = 0; k < 3; k++) { lists[k] = a->d_tuBy[k] + a->rowTuBy[k][r0]; n[k] = a->rowTuBy[k][r1] - a->rowTuBy[k][r0]; }
+    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r, lists, n) : launch_resid<uint16_t>(c, chroma, r, lists, n);
 }
 
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
@@ -232,7 +239,7 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     }
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
-    const int tu0 = a->rowTu[r0], ntu = a->rowTu[r1] - tu0;
+    const int ntu = a->rowTu[r1] - a->rowTu[r0];
     a->ev_valid = stages;
     CU_CHECK(cudaEventRecord(a->ev[0], c->stream));
     if ((stages & 1) && nj > 0)
@@ -274,17 +281,18 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     }
     else if (stages & 1) CU_CHECK(cudaEventRecord(a->ev[4], c->stream));
     CU_CHECK(cudaEventRecord(a->ev[1], c->stream));
-    if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, tu0, ntu)) return -1;
+    if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, r0, r1)) return -1;
     CU_CHECK(cudaEventRecord(a->ev[2], c->stream));
     if ((stages & 4) && ncu > 0)
     {
-        int blocks = ncu < c->sm_count * 8 ? ncu : c->sm_count * 8;
-        if (depth == 8) k_intra_search<uint8_t><<<blocks, 256, 0, c->stream>>>((const uint8_t*)(a->d_fenc + a->orgBytes), a->stride, a->d_cus + cu0, ncu, a->d_intra + (size_t)cu0 * 36);
-        else            k_intra_search<uint16_t><<<blocks, 256, 0, c->stream>>>((const uint16_t*)(a->d_fenc + a->orgBytes), a->stride, a->d_cus + cu0, ncu, a->d_intra + (size_t)cu0 * 36);
-        CU_LAUNCH_CHECK(c);
+        const int32_t* lists[4]; int n[4];
+        for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
+        const int e = depth == 8 ? launch_intra<uint8_t>(c, a->d_fenc + a->orgBytes, a->stride, a->d_cus, lists, n, a->d_intra)
+                                 : launch_intra<uint16_t>(c, a->d_fenc + a->orgBytes, a->stride, a->d_cus, lists, n, a->d_intra);
+        if (e) return -1;
     }
     CU_CHECK(cudaEventRecord(a->ev[3], c->stream));
-    if ((stages & 8) && ntu > 0 && an_residual(a, true, cu0, ncu, tu0, ntu)) return -1;
+    if ((stages & 8) && ntu > 0 && an_residual(a, true, cu0, ncu, r0, r1)) return -1;
     return 0;
 }
 
@@ -416,6 +424,7 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     void* bufs[] = { a->d_fenc, a->d_refTable, a->d_reconTable, a->d_field, a->d_mvcost, a->d_pus, a->d_cus, a->d_tus, a->d_cu_jobs, a->d_jobs,
                      a->d_me_out, a->d_me_packed, a->d_coef, a->d_cu_sse, a->d_cu_numsig, a->d_cu_ref, a->d_intra,
                      a->d_groups[0], a->d_groups[1], a->d_groups[2], a->d_grpJobs[0], a->d_grpJobs[1], a->d_grpJobs[2], a->d_tmaps, a->d_left, a->d_order,
+                     a->d_tuBy[0], a->d_tuBy[1], a->d_tuBy[2], a->d_cuBy[0], a->d_cuBy[1], a->d_cuBy[2], a->d_cuBy[3],
                      a->d_planeJobs[0], a->d_planeJobs[1], a->d_planeJobs[2] };
     for (void* b : bufs) cudaFree(b);
     for (int r = 0; r < a->p.numRefs; r++) cudaFree(a->d_refs[r]);

@@ -20,6 +20,10 @@ struct FrameGeometry
     // first PU job / CU / TU of every CTU row (+ one past the end): the lists are in CTU raster order, so a CTU-row
     // range [r0, r1) is one contiguous slice of each list (what a WPP row shard owns, frameencoder.cpp:850-868)
     int ctuRows; std::vector<int> rowJob, rowCu, rowTu;
+    // per-size work lists of the residual and intra stages, each launch of one block size reading only its own list: tuBy[k]
+    // = the TUs of luma size 8 << k (k = 0..2), cuBy[k] = the CUs of size 8 << k (k = 0..3), absolute indices in list order.
+    // rowTuBy[k] / rowCuBy[k] = first entry of every CTU row (+ one past the end), so a CTU-row range is one slice of each.
+    std::vector<int32_t> tuBy[3], cuBy[4]; std::vector<int> rowTuBy[3], rowCuBy[4];
     int64_t ncoef;
     // job groups of the shared-memory-window integer search (me_window.cuh): per (CTU, ref) the 64x64 CU's PUs, each 32x32
     // CU's PUs, and per 16x16 cell the PUs of the 16x16 CU and of its four 8x8 CUs.  grpJobs holds absolute job indices,
@@ -217,6 +221,23 @@ static inline void geometry_build(int W, int H, int stride, int nref, int rect, 
     for (int k = 0; k < 3; k++) g.rowGrp[k].push_back((int)g.grpFirst[k].size());
     g.rowJob.push_back((int)g.pus.size()); g.rowCu.push_back((int)g.cus.size()); g.rowTu.push_back((int)g.tus.size());
     g.ncoef = coefOff;
+    for (int r = 0; r < ctuH; r++)
+    {
+        for (int k = 0; k < 3; k++) g.rowTuBy[k].push_back((int)g.tuBy[k].size());
+        for (int k = 0; k < 4; k++) g.rowCuBy[k].push_back((int)g.cuBy[k].size());
+        for (int t = g.rowTu[r]; t < g.rowTu[r + 1]; t++)
+        {
+            const int S = g.cus[g.tus[t].cu].size;
+            g.tuBy[S >= 32 ? 2 : (S == 16 ? 1 : 0)].push_back(t);
+        }
+        for (int c = g.rowCu[r]; c < g.rowCu[r + 1]; c++)
+        {
+            const int S = g.cus[c].size;
+            g.cuBy[S == 64 ? 3 : (S == 32 ? 2 : (S == 16 ? 1 : 0))].push_back(c);
+        }
+    }
+    for (int k = 0; k < 3; k++) g.rowTuBy[k].push_back((int)g.tuBy[k].size());
+    for (int k = 0; k < 4; k++) g.rowCuBy[k].push_back((int)g.cuBy[k].size());
     // shape-sorted job order per CTU row: counting sort on (w, h) keys, stable (area descending, then width descending)
     g.order.resize(g.pus.size());
     for (int r = 0; r < ctuH; r++)

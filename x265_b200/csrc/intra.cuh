@@ -106,13 +106,14 @@ __device__ void intra_predict_block(const int16_t* nbs, int16_t* refbuf, P* __re
 }
 
 // 1:2:1 neighbour smoothing (intrapred.cpp:31-51), element i of 4N+1
-__device__ __forceinline__ int intra_filter_elem(const int16_t* s, int i, int N)
+template <typename T>
+__device__ __forceinline__ int intra_filter_elem(const T* s, int i, int N)
 {
     const int N2 = 2 * N, N4 = 4 * N;
-    if (i == 0) return (2 * s[0] + s[1] + s[N2 + 1] + 2) >> 2;
+    if (i == 0) return (2 * (int)s[0] + (int)s[1] + (int)s[N2 + 1] + 2) >> 2;
     if (i == N2 || i == N4) return s[i];
-    if (i == N2 + 1) return (2 * s[N2 + 1] + s[0] + s[N2 + 2] + 2) >> 2;
-    return (2 * s[i] + s[i - 1] + s[i + 1] + 2) >> 2;
+    if (i == N2 + 1) return (2 * (int)s[N2 + 1] + (int)s[0] + (int)s[N2 + 2] + 2) >> 2;
+    return (2 * (int)s[i] + (int)s[i - 1] + (int)s[i + 1] + 2) >> 2;
 }
 
 template <typename P>
@@ -229,13 +230,89 @@ __global__ void __launch_bounds__(256) k_intra_allangs_cta(int N, const P* __res
     }
 }
 
+// ---- packed angular prediction, shared by k_intra_allangs_packed and the frame analyser's intra search (frame.cuh) ----
+// Projected reference row of angular mode `mode` (2..34) of an N x N block in the vertical-family frame, kept as PIXELS:
+// refbuf[N + 2 + idx] = ref[idx], idx in [-N, 2N) (intrapred.cpp:120-160).  Built by the nl lanes li = 0..nl-1 of a group;
+// modes 10 / 26 (angle 0) need none.  The caller syncs the group before and after.
+template <typename P>
+__device__ __forceinline__ void intra_ang_ref(P* refbuf, const P* nbs, int N, int mode, int li, int nl)
+{
+    const bool hor = mode < 18;
+    const int angOff = hor ? 10 - mode : mode - 26, angle = c_angle[8 + angOff];
+    const int N2 = 2 * N, mainBase = hor ? N2 + 1 : 1, sideBase = hor ? 1 : N2 + 1, off = N + 1;
+    if (angle < 0)
+    {
+        const int nproj = -((N * angle) >> 5) - 1;
+        const int inv = c_invAngle[-angOff - 1];
+        for (int i = li; i < nproj; i += nl) refbuf[off + 1 + (-2 - i)] = nbs[sideBase - 1 + ((128 + (i + 1) * inv) >> 8)];
+        for (int i = li; i < N + 1; i += nl) refbuf[off + 1 + (-1 + i)] = (i == 0) ? nbs[0] : nbs[mainBase + i - 1];
+    }
+    else if (angle > 0)
+    {
+        for (int i = li; i < N2; i += nl) refbuf[off + 1 + i] = nbs[mainBase + i];
+    }
+}
+
+// Pixels c0 .. c0 + UW * 4 / sizeof(P) - 1 of row r of angular mode `mode` in the vertical-family frame (a horizontal mode's
+// block transposed), packed 4 (8-bit) / 2 (16-bit) per word.  From the projected row of intra_ang_ref: UW + 2 aligned words,
+// funnel shifts to the item's byte phase, then one DP4A (bytes p[k], p[k+1] against the weights (32 - f, f), + 16 in the
+// accumulator) or DP2A per pixel and one shift; f == 0 needs no special case: (32 p + 16) >> 5 == p.  Modes 10 / 26 (angle 0)
+// copy the main reference, with the edge filter on column 0 when bFilter.  refbuf must be 4-byte aligned and hold
+// 3N + 12 pixels (the words past the last used pixel are read and weighted by 0).
+template <typename P, int UW>
+__device__ __forceinline__ void intra_ang_item(const P* refbuf, const P* nbs, int N, int mode, int bFilter, int r, int c0, uint32_t o32[UW])
+{
+    constexpr int maxv = PixTraits<P>::maxv;
+    constexpr int ES = (int)sizeof(P), UPX = UW * 4 / ES;
+    const bool hor = mode < 18;
+    const int angOff = hor ? 10 - mode : mode - 26, angle = c_angle[8 + angOff];
+    const int N2 = 2 * N, mainBase = hor ? N2 + 1 : 1, sideBase = hor ? 1 : N2 + 1, off = N + 1;
+    if (angle == 0)
+    {
+        int v[UPX];
+#pragma unroll
+        for (int q = 0; q < UPX; q++) v[q] = nbs[mainBase + c0 + q];
+        if (bFilter && c0 == 0) v[0] = clip3i(0, maxv, (int)(int16_t)((int)nbs[mainBase] + (((int)nbs[sideBase + r] - (int)nbs[0]) >> 1)));
+#pragma unroll
+        for (int w = 0; w < UW; w++)
+            o32[w] = ES == 1 ? ((uint32_t)v[4 * w] | ((uint32_t)v[4 * w + 1] << 8) | ((uint32_t)v[4 * w + 2] << 16) | ((uint32_t)v[4 * w + 3] << 24))
+                             : ((uint32_t)v[(2 * w) % UPX] | ((uint32_t)v[(2 * w + 1) % UPX] << 16));
+        return;
+    }
+    const int pos = (r + 1) * angle, o = pos >> 5, f = pos & 31;
+    const uint32_t W = (uint32_t)(32 - f) | ((uint32_t)f << 8);
+    const unsigned bo = (unsigned)(off + 1 + o + c0) * ES;
+    const uint32_t* wp = (const uint32_t*)refbuf + (bo >> 2);
+    const unsigned sh = (bo & 3u) * 8u;
+    uint32_t wd[UW + 2], x[UW + 1];
+#pragma unroll
+    for (int w = 0; w < UW + 2; w++) wd[w] = wp[w];
+#pragma unroll
+    for (int w = 0; w < UW + 1; w++) x[w] = __funnelshift_r(wd[w], wd[w + 1], sh);
+#pragma unroll
+    for (int w = 0; w < UW; w++)
+    {
+        if (ES == 1)
+        {
+            const uint32_t p0 = (uint32_t)dp4a_us(x[w], W, 16) >> 5, p1 = (uint32_t)dp4a_us(x[w], W << 8, 16) >> 5;
+            const uint32_t p2 = (uint32_t)dp4a_us(x[w], W << 16, 16) >> 5;
+            const uint32_t p3 = (uint32_t)dp4a_us(__funnelshift_r(x[w], x[w + 1], 24), W, 16) >> 5;
+            o32[w] = p0 | (p1 << 8) | (p2 << 16) | (p3 << 24);
+        }
+        else
+        {
+            const uint32_t p0 = (uint32_t)dp2a_lo_ss(x[w], W, 16) >> 5;
+            const uint32_t p1 = (uint32_t)dp2a_lo_ss(__funnelshift_r(x[w], x[w + 1], 16), W, 16) >> 5;
+            o32[w] = p0 | (p1 << 16);
+        }
+    }
+}
+
 // all-angs on packed pixels: same per-pixel arithmetic as k_intra_allangs_cta, issued 4 (8-bit) / 2 (16-bit) pixels per word.
 // The CTA kernel above spends ~45 instructions per 4 pixels (two shared loads, two IMADs, shift and select per pixel, the
 // packing) and keeps half a warp idle on a 16x16 block (a mode has 16 row units there): issue bound.  Here
 //   * neighbours and the projected reference row are kept as PIXELS in shared memory, a work item is a 16-byte piece of an
-//     output row (a whole row up to 16 / 8 pixels): UW + 2 aligned words, funnel shifts to the item's byte phase, then one
-//     DP4A (bytes p[k], p[k+1] against the weights (32 - f, f), + 16 in the accumulator) or DP2A per pixel and one shift;
-//     f == 0 needs no special case: (32 p + 16) >> 5 == p;
+//     output row (a whole row up to 16 / 8 pixels), computed by intra_ang_item;
 //   * a warp runs 32 / items-per-mode modes side by side (two for a 16x16 8-bit block, four for 8x8), each with its own
 //     reference row, so all lanes are busy for every block size.
 // Modes 10 / 26 (angle 0: a copy of the main reference plus the edge filter) stay scalar.
@@ -243,18 +320,16 @@ template <typename P, int UW>
 __global__ void __launch_bounds__(256) k_intra_allangs_packed(int N, const P* __restrict__ refp, const P* __restrict__ filtp, int64_t nb_pitch,
                                                               P* __restrict__ dst, int bLuma, int n)
 {
-    constexpr int maxv = PixTraits<P>::maxv;
     constexpr int ES = (int)sizeof(P), UPX = UW * 4 / ES;          // pixels per work item
     __shared__ __align__(16) P s_nb[2][136];
     __shared__ __align__(16) P s_ref[8][8][136];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int lg = 31 - __clz(N), N2 = 2 * N;
+    const int lg = 31 - __clz(N);
     const int cpr = N / UPX, ipm = N * cpr;                        // items per row / per mode (both powers of two, ipm <= 64)
     const int G = ipm >= 32 ? 1 : 32 / ipm;                        // modes a warp runs side by side
     const int g = ipm >= 32 ? 0 : lane / ipm, li = ipm >= 32 ? lane : lane - g * ipm, lstep = ipm >= 32 ? 32 : ipm;
     const int slot = warp * G + g, nslots = 8 * G, rounds = (33 + nslots - 1) / nslots;
     P* refbuf = s_ref[warp][g];
-    const int off = N + 1;
     for (int j = blockIdx.x; j < n; j += gridDim.x)
     {
         __syncthreads();
@@ -269,22 +344,8 @@ __global__ void __launch_bounds__(256) k_intra_allangs_packed(int N, const P* __
             const int mode = 2 + slot + k * nslots;
             const bool active = mode < 35;
             const P* nbs = s_nb[active && intra_use_filtered(mode, N) ? 1 : 0];
-            const bool hor = mode < 18;
-            const int angOff = hor ? 10 - mode : mode - 26;
-            const int angle = active ? c_angle[8 + angOff] : 0;
-            const int mainBase = hor ? N2 + 1 : 1, sideBase = hor ? 1 : N2 + 1;
             __syncwarp();
-            if (active && angle < 0)
-            {
-                const int nproj = -((N * angle) >> 5) - 1;
-                const int inv = c_invAngle[-angOff - 1];
-                for (int i = li; i < nproj; i += lstep) refbuf[off + 1 + (-2 - i)] = nbs[sideBase - 1 + ((128 + (i + 1) * inv) >> 8)];
-                for (int i = li; i < N + 1; i += lstep) refbuf[off + 1 + (-1 + i)] = (i == 0) ? nbs[0] : nbs[mainBase + i - 1];
-            }
-            else if (active && angle > 0)
-            {
-                for (int i = li; i < N2; i += lstep) refbuf[off + 1 + i] = nbs[mainBase + i];
-            }
+            if (active) intra_ang_ref<P>(refbuf, nbs, N, mode, li, lstep);
             __syncwarp();
             if (active)
             {
@@ -293,47 +354,7 @@ __global__ void __launch_bounds__(256) k_intra_allangs_packed(int N, const P* __
                 {
                     const int r = it / cpr, c0 = (it - r * cpr) * UPX;
                     uint32_t o32[UW];
-                    if (angle == 0)
-                    {
-                        int v[UPX];
-#pragma unroll
-                        for (int q = 0; q < UPX; q++) v[q] = nbs[mainBase + c0 + q];
-                        if (bLuma && c0 == 0) v[0] = clip3i(0, maxv, (int)(int16_t)((int)nbs[mainBase] + (((int)nbs[sideBase + r] - (int)nbs[0]) >> 1)));
-#pragma unroll
-                        for (int w = 0; w < UW; w++)
-                            o32[w] = ES == 1 ? ((uint32_t)v[4 * w] | ((uint32_t)v[4 * w + 1] << 8) | ((uint32_t)v[4 * w + 2] << 16) | ((uint32_t)v[4 * w + 3] << 24))
-                                             : ((uint32_t)v[(2 * w) % UPX] | ((uint32_t)v[(2 * w + 1) % UPX] << 16));
-                    }
-                    else
-                    {
-                        const int pos = (r + 1) * angle, o = pos >> 5, f = pos & 31;
-                        const uint32_t W = (uint32_t)(32 - f) | ((uint32_t)f << 8);
-                        const unsigned bo = (unsigned)(off + 1 + o + c0) * ES;
-                        const uint32_t* wp = (const uint32_t*)refbuf + (bo >> 2);
-                        const unsigned sh = (bo & 3u) * 8u;
-                        uint32_t wd[UW + 2], x[UW + 1];
-#pragma unroll
-                        for (int w = 0; w < UW + 2; w++) wd[w] = wp[w];
-#pragma unroll
-                        for (int w = 0; w < UW + 1; w++) x[w] = __funnelshift_r(wd[w], wd[w + 1], sh);
-#pragma unroll
-                        for (int w = 0; w < UW; w++)
-                        {
-                            if (ES == 1)
-                            {
-                                const uint32_t p0 = (uint32_t)dp4a_us(x[w], W, 16) >> 5, p1 = (uint32_t)dp4a_us(x[w], W << 8, 16) >> 5;
-                                const uint32_t p2 = (uint32_t)dp4a_us(x[w], W << 16, 16) >> 5;
-                                const uint32_t p3 = (uint32_t)dp4a_us(__funnelshift_r(x[w], x[w + 1], 24), W, 16) >> 5;
-                                o32[w] = p0 | (p1 << 8) | (p2 << 16) | (p3 << 24);
-                            }
-                            else
-                            {
-                                const uint32_t p0 = (uint32_t)dp2a_lo_ss(x[w], W, 16) >> 5;
-                                const uint32_t p1 = (uint32_t)dp2a_lo_ss(__funnelshift_r(x[w], x[w + 1], 16), W, 16) >> 5;
-                                o32[w] = p0 | (p1 << 16);
-                            }
-                        }
-                    }
+                    intra_ang_item<P, UW>(refbuf, nbs, N, mode, bLuma, r, c0, o32);
                     P* d = out + (r << lg) + c0;
                     if (UW == 4)      *(uint4*)d = make_uint4(o32[0], o32[1], o32[2], o32[3]);
                     else if (UW == 2) *(uint2*)d = make_uint2(o32[0], o32[1]);

@@ -5,9 +5,9 @@
 //   vector read as eighth-pel) -> sub_ps -> dct -> quant -> dequant_normal -> idct / DC shortcut -> add_ps -> sse_pp
 //   (search.cpp:3178 estimateResidualQT, search.cpp:2990-3080; quant.cpp:397-470, :543-605, non-RDOQ path).
 // The reference and vector are the lowest ME cost of the CU's 2Nx2N jobs, ties to the lowest index.  The MC is pc_predict
-// (predcost.cuh).  A job group of TPJ threads takes one (TU, plane) item at a time: luma TUs take a 256-thread CTA each,
-// chroma TUs of 4 and 8 a WARP each (four per CTA, private shared tiles, warp barriers only), chroma TUs of 16 a 128-thread
-// CTA each.
+// (predcost.cuh).  A job group of TPJ threads takes one (TU, plane) item at a time, and every launch reads the list of one
+// luma TU size (geometry.h tuBy): TUs of 4 and 8 take a WARP each (four per CTA, private shared tiles, warp barriers only),
+// TUs of 16 a 128-thread CTA each, luma TUs of 32 a 256-thread CTA each.
 #pragma once
 #include "common.cuh"
 #include "predcost.cuh"
@@ -55,20 +55,21 @@ __device__ __forceinline__ T resid_group_sum(T v, T* s_red)
 }
 
 // Per-plane inputs and outputs of the stage.  NPL planes (1 luma, 2 Cb / Cr) share the stride and the TU list; levels and
-// recon of a plane share its geometry.  recon = origin pointers [NPL * depthIdx + plane]; cu_sse / cu_numsig are
-// [NPL * cu + plane] and accumulate; cu_ref (luma) receives the chosen reference, or is null.
+// recon of a plane share its geometry.  tus is the whole TU table, tul the launch's slice of one per-size list (ntu
+// entries).  recon = origin pointers [NPL * depthIdx + plane]; cu_sse / cu_numsig are [NPL * cu + plane] and accumulate;
+// cu_ref (luma) receives the chosen reference, or is null.
 struct ResidArgs
 {
     const void* fenc[2]; const void* const* refs[2]; int16_t* coef[2]; int qp[2];
     int stride; void* const* recon;
-    const CuDesc* cus; const TuDesc* tus; int ntu; const int32_t* cu_jobs; int numRefs; const int32_t* me_out;
+    const CuDesc* cus; const TuDesc* tus; const int32_t* tul; int ntu; const int32_t* cu_jobs; int numRefs; const int32_t* me_out;
     unsigned long long* cu_sse; uint32_t* cu_numsig; int32_t* cu_ref;
 };
 
-// Item j of [0, NPL * ntu) = plane j % NPL of TU j / NPL.  NT = 8 is the luma plane, NT = 4 the two chroma planes at half
-// resolution.  A launch takes the items whose TU is minSize..MAXS wide; a sibling launch owns the others.
+// Item j of [0, NPL * ntu) = plane j % NPL of TU tul[j / NPL].  NT = 8 is the luma plane, NT = 4 the two chroma planes at half
+// resolution.  Every TU of the list is at most MAXS wide in the launch's planes.
 template <typename P, int TPJ, int MAXS, int NT>
-__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const ResidArgs a, int minSize)
+__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const ResidArgs a)
 {
     constexpr int DEPTH = PixTraits<P>::depth, maxv = PixTraits<P>::maxv;
     constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ, NPL = NT == 8 ? 1 : 2, SUB = NPL - 1;
@@ -90,12 +91,11 @@ __global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const Res
     int8_t* M = s_mat[grp];
     for (int j = blockIdx.x * JPB + grp; j < NPL * a.ntu; j += gridDim.x * JPB)
     {
-        const TuDesc tu = a.tus[j / NPL];
+        const TuDesc tu = a.tus[a.tul[j / NPL]];
         const int plane = j % NPL;
         const CuDesc cu = a.cus[tu.cu];
         const PlaneTu pt = geometry_plane_tu(cu, tu, SUB);
         const int T = pt.size;
-        if (T < minSize || T > MAXS) continue;
         const int lg = 31 - __clz(T), N = T * T;
         int best = 0, bcost = 0x7fffffff;
         for (int r = 0; r < a.numRefs; r++)
@@ -209,20 +209,29 @@ __global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const Res
 }
 
 template <typename P, int TPJ, int MAXS, int NT>
-static int resid_launch(x265cu_ctx* c, int blocks, int minSize, const ResidArgs& a)
+static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a)
 {
-    k_cu_residual<P, TPJ, MAXS, NT><<<blocks, TPJ > 128 ? TPJ : 128, 0, c->stream>>>(a, minSize);
+    constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ;
+    const int items = (NT == 8 ? 1 : 2) * a.ntu;
+    if (items == 0) return 0;
+    k_cu_residual<P, TPJ, MAXS, NT><<<min((items + JPB - 1) / JPB, c->sm_count * maxPerSm), TPJ > 128 ? TPJ : 128, 0, c->stream>>>(a);
     CU_LAUNCH_CHECK(c);
     return 0;
 }
 
-// luma: a CTA per TU, at most 8 per SM; chroma: the warp launch (TUs of 4 and 8) and the CTA launch (TUs of 16) over the
-// same (TU, plane) list, at most 16 CTAs per SM each
+// One launch per luma TU size, each over its own list (lists[k] = TUs of luma size 8 << k, n[k] entries): luma TUs of 8 a
+// warp each, of 16 a 128-thread CTA, of 32 a 256-thread CTA (at most 8 per SM); chroma TUs of 4 and 8 a warp each, of 16 a
+// 128-thread CTA; at most 16 CTAs per SM otherwise
 template <typename P>
-static int launch_resid(x265cu_ctx* c, bool chroma, const ResidArgs& a)
+static int launch_resid(x265cu_ctx* c, bool chroma, ResidArgs a, const int32_t* const lists[3], const int n[3])
 {
-    if (!chroma) return resid_launch<P, 256, 32, 8>(c, min(a.ntu, c->sm_count * 8), 0, a);
-    const int n = 2 * a.ntu, maxb = c->sm_count * 16;
-    if (resid_launch<P, 32, 8, 4>(c, min((n + 3) / 4, maxb), 0, a)) return -1;
-    return resid_launch<P, 128, 16, 4>(c, min(n, maxb), 16, a);
+    for (int k = 0; k < 3; k++)
+    {
+        a.tul = lists[k]; a.ntu = n[k];
+        const int e = chroma ? (k < 2 ? resid_launch<P, 32, 8, 4>(c, 16, a) : resid_launch<P, 128, 16, 4>(c, 16, a))
+                             : (k == 0 ? resid_launch<P, 32, 8, 8>(c, 16, a) : k == 1 ? resid_launch<P, 128, 16, 8>(c, 16, a)
+                                                                                     : resid_launch<P, 256, 32, 8>(c, 8, a));
+        if (e) return -1;
+    }
+    return 0;
 }
