@@ -477,6 +477,71 @@ int x265cu_lookahead_weights_analyse(x265cu_ctx*, int depth, const void* fencBuf
                                      void* wbuf_dev, int64_t planesize, int stride, int width, int lines, int64_t padoffset,
                                      const int32_t* intraCost_host, const uint64_t* stats, int* wp_out);
 
+/* Adaptive quantisation: LookaheadTLD::calcAdaptiveQuantFrame (slicetype.cpp:444-694), split as cuTree is.  The per-block
+ * integer work (acEnergyCu, :49-84, 256-275) is x265cu_aq_energy on the device, exact in any order; the float decision is
+ * x265cu_aq_finish, a literal restatement on the host (its pow / log2 are the host's libm, and the library's host code is
+ * compiled without FMA contraction or fast-math, so it equals a reference built with the same libm bit for bit).
+ *
+ * Geometry, with L = 8 at qgSize 8 and 16 otherwise, w8 = (W / 2 + 7) >> 3, h8 = (H / 2 + 7) >> 3 (Lowres::maxBlocksInRow /
+ * maxBlocksInCol):
+ *   energy grid   ceil(W / L) x ceil(H / L) blocks, raster order: the reference's loops over blockY / blockX step L
+ *   blockCount    4 * w8 * h8 at qgSize 8, else w8 * h8: the length of qpAqOffset / invQscaleFactor / blockVariance /
+ *                 quantOffsets (Lowres::create, Frame::create); it can exceed the energy grid at qgSize 8 */
+
+/* energy[ceil(W / L) * ceil(H / L)] (uint32, device) receives acEnergyCu of every block; totals[3][2] (uint64, device)
+ * receives, per plane, the sums of var's `sum` and `ssd` over all blocks: what one acEnergyCu pass adds to wp_sum[plane] /
+ * wp_ssd[plane].  Luma is var 16x16 (shift 8), or 8x8 (shift 6) at qgSize 8; 4:2:0 chroma is var 8x8 (shift 6), or 4x4
+ * (shift 4), at (blockX >> 1, blockY >> 1).  Planes are device pointers at pixel (0,0), strides in elements; cb = cr = NULL
+ * is 4:0:0 (luma only, chroma totals 0).  Edge blocks: reads past the picture take the nearest in-picture sample (clamped
+ * coordinates), which is what the reference reads from PicYuv's replicated padding (picyuv.cpp:209-234), so the planes
+ * need no margins.  Returns -1 before any launch (x265cu_last_error) for a depth other than 8 / 10, a qgSize other than
+ * 8 / 16 / 32 / 64, a non-positive or odd width or height, a stride smaller than the row, a NULL luma or output pointer, or
+ * only one NULL chroma pointer.  Runs on the context's stream. */
+int x265cu_aq_energy(x265cu_ctx*, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                     int width, int height, int qgSize, uint32_t* energy_dev, uint64_t* totals_dev);
+
+typedef struct {
+    int32_t aqMode;             /* rc.aqMode: 0 NONE, 1 VARIANCE, 2 AUTO_VARIANCE, 3 AUTO_VARIANCE_BIASED (4 EDGE refused) */
+    int32_t qgSize;             /* rc.qgSize: 8, 16, 32 or 64 */
+    int32_t weightp;            /* bEnableWeightedPred || bEnableWeightedBiPred */
+    int32_t variance;           /* bDynamicRefine || bEnableFades: blockVariance / frameVariance */
+    int32_t hevcAq, hdr10Opt, aqMotion;   /* rc.hevcAq, bHDR10Opt, bAQMotion: refused when set (they stay on the host) */
+    int32_t reserved;
+    double aqStrength;          /* rc.aqStrength */
+    const float* quantOffsets;  /* x265_picture::quantOffsets (blockCount floats, frame.cpp:141-146) or NULL */
+} x265cu_aq_params;
+
+/* Host outputs of x265cu_aq_finish; each may be NULL.  The arrays are in / out: entries the reference does not write keep
+ * their contents (aqMode 0 writes no offsets; the main path writes only the energy grid's entries).  qpAqOffset holds what
+ * the reference stores in both Lowres::qpAqOffset and qpCuTreeOffset.  invQscaleFactor8x8 (w8 * h8, qgSize 8) is the
+ * reduction of :637-650, which reads invQscaleFactor with the reference's stride widthInCU * 2; it needs invQscaleFactor. */
+typedef struct {
+    double* qpAqOffset;             /* blockCount */
+    int32_t* invQscaleFactor;       /* blockCount, x265_exp2fix8 of the offsets */
+    int32_t* invQscaleFactor8x8;    /* w8 * h8, qgSize 8 only */
+    uint64_t* wp_sum;               /* [3]: Lowres::wp_sum after the call */
+    uint64_t* wp_ssd;               /* [3]: Lowres::wp_ssd after the call (weightp's correction applied, :653-676) */
+    uint32_t* blockVariance;        /* blockCount, with variance */
+    double* frameVariance;          /* with variance */
+} x265cu_aq_out;
+
+/* calcAdaptiveQuantFrame's decision (:466-693) on x265cu_aq_energy's energies and totals (host copies); needs no device.
+ * The caller skips the reference's `rc.bStatRead && cuTree && IS_REFERENCED` case (:473), which computes no offsets.
+ * Returns -1 with x265cu_last_error for aq-mode 4 (EDGE: Sobel and atan2 in float), hevc-aq, HDR10 opt and aq-motion,
+ * which stay on the host; for bad depth / qgSize / geometry; for NULL energy or totals; for invQscaleFactor8x8 without
+ * invQscaleFactor; and for variance with weightp when weightp's rounding of the picture to ((W + 8) >> 4) << 4 columns /
+ * rows changes the grid the fades pass walks (:664-665, 678-693; for sides that are multiples of 8, qgSize 8 with W or
+ * H % 16 == 8). */
+int x265cu_aq_finish(int depth, int width, int height, const x265cu_aq_params* params, const uint32_t* energy,
+                     const uint64_t* totals, const x265cu_aq_out* out);
+
+/* The whole of calcAdaptiveQuantFrame for one picture: x265cu_aq_energy, the download of energies and totals, x265cu_aq_finish
+ * into `out` (may be NULL) and, when aqMode != 0 and invQscale_dev is not NULL, the upload of invQscaleFactor (w8 * h8
+ * entries, or invQscaleFactor8x8 at qgSize 8) into invQscale_dev: the array x265cu_la_intra_job.invQscale,
+ * x265cu_la_job.invQscale and x265cu_cutree_frame.invQscale read.  Synchronises the context's stream. */
+int x265cu_aq_frame(x265cu_ctx*, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                    int width, int height, const x265cu_aq_params* params, int32_t* invQscale_dev, const x265cu_aq_out* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libx265cu.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-shared"]
+              "-Xcompiler", "-fPIC", "-shared",
+              "-Xcompiler", "-ffp-contract=off"]          # host code: x265cu_aq_finish rounds as the reference does
 
 
 def _newest_source():

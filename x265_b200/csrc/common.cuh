@@ -22,6 +22,7 @@ struct x265cu_ctx
     cudaEvent_t me_ev[4];               // boundaries of the three ME launches of the last x265cu_me_batch / analyser run
     void* d_sao_lines; size_t sao_lines_bytes; // CTU edge lines saved by x265cu_sao_apply_frame before it filters in place
     void* d_cutree; size_t cutree_bytes;       // x265cu_cutree: one level's propagate amounts and the levels' overflow flags
+    void* d_aq; size_t aq_bytes;               // x265cu_aq_frame: the energies and plane totals of one picture
 };
 
 void x265cu_set_error(const char* what, cudaError_t e, const char* file, int line);

@@ -12,6 +12,7 @@
 #include "frame.cuh"
 #include "resid.cuh"
 #include "lookahead.cuh"
+#include "aq.cuh"
 #include <math.h>
 #include <mutex>
 #include <vector>
@@ -39,7 +40,7 @@ int x265cu_device_count(void)
 static void ctx_release(x265cu_ctx* c)
 {
     if (c->h_stage) cudaFreeHost(c->h_stage);
-    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state); cudaFree(c->d_sao_lines); cudaFree(c->d_cutree);
+    cudaFree(c->d_stage); cudaFree(c->d_counter); cudaFree(c->d_me_state); cudaFree(c->d_sao_lines); cudaFree(c->d_cutree); cudaFree(c->d_aq);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
     for (int i = 0; i < 4; i++) if (c->me_ev[i]) cudaEventDestroy(c->me_ev[i]);
@@ -892,4 +893,261 @@ extern "C" int x265cu_cutree(x265cu_ctx* c, x265cu_cutree_frame* frames, int num
     for (int f = 0; f <= numframes; f++)
         frames[f].propagateCost = pc[f];
     return nfinish;
+}
+
+// ---------------- adaptive quantisation: calcAdaptiveQuantFrame (slicetype.cpp:444-694) ----------------
+// the argument rules of x265cu_aq_energy; NULL when they hold
+static const char* aq_energy_check(int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                                   int width, int height, int qgSize, const void* energy, const void* totals)
+{
+    if (depth != 8 && depth != 10) return "depth must be 8 or 10";
+    if (qgSize != 8 && qgSize != 16 && qgSize != 32 && qgSize != 64) return "qgSize must be 8, 16, 32 or 64";
+    if (width <= 0 || height <= 0 || (width & 1) || (height & 1)) return "width and height must be positive and even";
+    if (!luma || !energy || !totals) return "NULL luma plane or output";
+    if (!cb != !cr) return "give both chroma planes or neither";
+    if (stride < width || (cb && cstride < width / 2)) return "stride smaller than the row";
+    return NULL;
+}
+
+static int aq_energy_launch(x265cu_ctx* c, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                            int width, int height, int qgSize, uint32_t* energy, uint64_t* totals)
+{
+    const int L = qgSize == 8 ? 8 : 16;
+    const int bw = (width + L - 1) / L, nb = bw * ((height + L - 1) / L);
+    CU_CHECK(cudaMemsetAsync(totals, 0, 6 * sizeof(uint64_t), c->stream));
+    const dim3 grid((nb + AQ_WARPS - 1) / AQ_WARPS), block(AQ_WARPS * 32);
+    unsigned long long* t = (unsigned long long*)totals;
+#define AQ_LAUNCH(P, LB) k_aq_energy<P, LB><<<grid, block, 0, c->stream>>>((const P*)luma, stride, (const P*)cb, (const P*)cr, \
+                                                                           cstride, width, height, bw, nb, energy, t)
+    if (depth == 8) { if (L == 8) AQ_LAUNCH(uint8_t, 8); else AQ_LAUNCH(uint8_t, 16); }
+    else            { if (L == 8) AQ_LAUNCH(uint16_t, 8); else AQ_LAUNCH(uint16_t, 16); }
+#undef AQ_LAUNCH
+    CU_LAUNCH_CHECK(c);
+    return 0;
+}
+
+extern "C" int x265cu_aq_energy(x265cu_ctx* c, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                                int width, int height, int qgSize, uint32_t* energy_dev, uint64_t* totals_dev)
+{
+    const char* bad = aq_energy_check(depth, luma, stride, cb, cr, cstride, width, height, qgSize, energy_dev, totals_dev);
+    if (bad)
+    {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "x265cu_aq_energy: %s", bad);
+        x265cu_set_error(msg, cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    cudaSetDevice(c->device);
+    return aq_energy_launch(c, depth, luma, stride, cb, cr, cstride, width, height, qgSize, energy_dev, totals_dev);
+}
+
+// x265_exp2fix8 (common/common.cpp:96-103); its table is round((2^(i/64) - 1) * 256)
+static int aq_exp2fix8(double x)
+{
+    static const struct Lut { uint8_t v[64]; Lut() { for (int i = 0; i < 64; i++) v[i] = (uint8_t)floor((exp2(i / 64.0) - 1) * 256 + 0.5); } } lut;
+    int i = (int)(x * (-64.f / 6.f) + 512.5f);
+    if (i < 0) return 0;
+    if (i > 1023) return 0xffff;
+    return (lut.v[i & 63] + 256) << (i >> 6) >> 8;
+}
+
+// the rules of x265cu_aq_finish; NULL when they hold
+static const char* aq_finish_check(int depth, int width, int height, const x265cu_aq_params* p, const void* energy,
+                                   const void* totals, const x265cu_aq_out* out)
+{
+    if (!p) return "NULL parameters";
+    if (p->aqMode == 4) return "aq-mode 4 (EDGE) stays on the host";
+    if (p->aqMode < 0 || p->aqMode > 4) return "aqMode must be 0..3";
+    if (p->hevcAq) return "hevc-aq stays on the host";
+    if (p->hdr10Opt) return "HDR10 opt stays on the host";
+    if (p->aqMotion) return "aq-motion stays on the host";
+    if (depth != 8 && depth != 10) return "depth must be 8 or 10";
+    if (p->qgSize != 8 && p->qgSize != 16 && p->qgSize != 32 && p->qgSize != 64) return "qgSize must be 8, 16, 32 or 64";
+    if (width <= 0 || height <= 0 || (width & 1) || (height & 1)) return "width and height must be positive and even";
+    if (!energy || !totals) return "NULL energies or totals";
+    if (out && out->invQscaleFactor8x8 && !out->invQscaleFactor) return "invQscaleFactor8x8 needs invQscaleFactor";
+    if (p->variance && p->weightp)
+    {
+        const int L = p->qgSize == 8 ? 8 : 16;
+        const int wp = ((width + 8) >> 4) << 4, hp = ((height + 8) >> 4) << 4;
+        if ((wp + L - 1) / L != (width + L - 1) / L || (hp + L - 1) / L != (height + L - 1) / L)
+            return "with weightp the fades pass walks a grid other than the energy grid; it stays on the host";
+    }
+    return NULL;
+}
+
+// slicetype.cpp:466-693 on the energies (one acEnergyCu per grid block, raster order) and one pass's plane totals
+static void aq_finish(int depth, int W, int H, const x265cu_aq_params* p, const uint32_t* energy, const uint64_t* totals,
+                      const x265cu_aq_out* o)
+{
+    const int qg = p->qgSize, L = qg == 8 ? 8 : 16;
+    const int bw = (W + L - 1) / L, bh = (H + L - 1) / L, nb = bw * bh;
+    const int w8 = ((W / 2) + 7) >> 3, h8 = ((H / 2) + 7) >> 3;
+    const int blockCount = qg == 8 ? (2 * w8) * (2 * h8) : w8 * h8;
+    const float modeOneConst = qg == 8 ? 11.427f : 14.427f, modeTwoConst = qg == 8 ? 8.f : 11.f;
+    const float* quantOffsets = p->quantOffsets;
+    std::vector<double> qpBuf, cut;
+    std::vector<int32_t> invqBuf;
+    double* qpAq = o->qpAqOffset;
+    int32_t* invq = o->invQscaleFactor;
+    if (!qpAq) { qpBuf.assign(blockCount, 0.0); qpAq = qpBuf.data(); }
+    if (!invq) { invqBuf.assign(blockCount, 0); invq = invqBuf.data(); }
+    uint64_t wsum[3] = { 0, 0, 0 }, wssd[3] = { 0, 0, 0 };
+    auto add_pass = [&]() { for (int i = 0; i < 3; i++) { wsum[i] += totals[2 * i]; wssd[i] += totals[2 * i + 1]; } };
+
+    if (p->aqMode == 0 || p->aqStrength == 0)
+    {
+        if (p->aqMode && p->aqStrength == 0)
+            for (int i = 0; i < blockCount; i++)
+            {
+                qpAq[i] = quantOffsets ? quantOffsets[i] : 0;
+                invq[i] = quantOffsets ? aq_exp2fix8(qpAq[i]) : 256;
+            }
+        if (p->weightp)
+            add_pass();
+    }
+    else
+    {
+        add_pass();                                  // modes 2 / 3: the first loop's acEnergyCu; mode 1: the second's
+        double avg_adj_pow2 = 0, avg_adj = 0, qp_adj = 0, bias_strength = 0.f, strength = 0.f;
+        if (p->aqMode == 2 || p->aqMode == 3)
+        {
+            cut.resize(nb);
+            const double bit_depth_correction = 1.f / (1 << (2 * (depth - 8)));
+            for (int b = 0; b < nb; b++)
+            {
+                qp_adj = pow(energy[b] * bit_depth_correction + 1, 0.1);
+                cut[b] = qp_adj;
+                avg_adj += qp_adj;
+                avg_adj_pow2 += qp_adj * qp_adj;
+            }
+            avg_adj /= blockCount;                   // blockCount, not the number of loop iterations
+            avg_adj_pow2 /= blockCount;
+            strength = p->aqStrength * avg_adj;
+            avg_adj = avg_adj - 0.5f * (avg_adj_pow2 - modeTwoConst) / avg_adj;
+            bias_strength = p->aqStrength;
+        }
+        else
+            strength = p->aqStrength * 1.0397f;
+        for (int b = 0; b < nb; b++)
+        {
+            if (p->aqMode == 3)
+            {
+                qp_adj = cut[b];
+                qp_adj = strength * (qp_adj - avg_adj) + bias_strength * (1.f - modeTwoConst / (qp_adj * qp_adj));
+            }
+            else if (p->aqMode == 2)
+            {
+                qp_adj = cut[b];
+                qp_adj = strength * (qp_adj - avg_adj);
+            }
+            else
+            {
+                const uint32_t e = energy[b];
+                qp_adj = strength * (log2(e > 1u ? e : 1u) - (modeOneConst + 2 * (depth - 8)));
+            }
+            if (quantOffsets)
+                qp_adj += quantOffsets[b];
+            qpAq[b] = qp_adj;
+            invq[b] = aq_exp2fix8(qp_adj);
+        }
+    }
+    if (qg == 8 && o->invQscaleFactor8x8)            // the full-res stride is widthInCU * 2, whatever the loop wrote
+        for (int cuY = 0; cuY < h8; cuY++)
+            for (int cuX = 0; cuX < w8; cuX++)
+            {
+                const int i = cuX * 2 + cuY * w8 * 4;
+                o->invQscaleFactor8x8[cuX + cuY * w8] = (invq[i] + invq[i + 1] + invq[i + 2 * w8] + invq[i + 2 * w8 + 1]) / 4;
+            }
+    int maxCol = W, maxRow = H;
+    if (p->weightp)
+    {
+        maxCol = ((maxCol + 8) >> 4) << 4;
+        maxRow = ((maxRow + 8) >> 4) << 4;
+        const int width[3] = { maxCol, maxCol >> 1, maxCol >> 1 }, height[3] = { maxRow, maxRow >> 1, maxRow >> 1 };
+        for (int i = 0; i < 3; i++)                  // uint64, wraps as the reference's does (4:0:0: chroma stays 0)
+            wssd[i] = wssd[i] - (wsum[i] * wsum[i] + (width[i] * height[i]) / 2) / (width[i] * height[i]);
+    }
+    if (p->variance)                                 // the fades pass: a second acEnergyCu pass, after the correction
+    {
+        uint64_t rowVariance = 0;                    // never reset between rows
+        double frameVariance = 0;
+        for (int by = 0; by < bh; by++)
+        {
+            for (int bx = 0; bx < bw; bx++)
+            {
+                const uint32_t e = energy[by * bw + bx];
+                if (o->blockVariance) o->blockVariance[by * bw + bx] = e;
+                rowVariance += e;
+            }
+            frameVariance += (rowVariance / maxCol);
+        }
+        frameVariance /= maxRow;
+        if (o->frameVariance) *o->frameVariance = frameVariance;
+        add_pass();
+    }
+    for (int i = 0; i < 3; i++)
+    {
+        if (o->wp_sum) o->wp_sum[i] = wsum[i];
+        if (o->wp_ssd) o->wp_ssd[i] = wssd[i];
+    }
+}
+
+static int aq_refuse(const char* fn, const char* why)
+{
+    char msg[200];
+    snprintf(msg, sizeof(msg), "%s: %s", fn, why);
+    x265cu_set_error(msg, cudaErrorInvalidValue, __FILE__, __LINE__);
+    return -1;
+}
+
+extern "C" int x265cu_aq_finish(int depth, int width, int height, const x265cu_aq_params* p, const uint32_t* energy,
+                                const uint64_t* totals, const x265cu_aq_out* out)
+{
+    const char* bad = aq_finish_check(depth, width, height, p, energy, totals, out);
+    if (bad) return aq_refuse("x265cu_aq_finish", bad);
+    const x265cu_aq_out none = {};
+    aq_finish(depth, width, height, p, energy, totals, out ? out : &none);
+    return 0;
+}
+
+extern "C" int x265cu_aq_frame(x265cu_ctx* c, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
+                               int width, int height, const x265cu_aq_params* p, int32_t* invQscale_dev, const x265cu_aq_out* out)
+{
+    const char* bad = p ? aq_energy_check(depth, luma, stride, cb, cr, cstride, width, height, p->qgSize, luma, luma) : NULL;
+    if (!bad) bad = aq_finish_check(depth, width, height, p, luma, luma, out);
+    if (bad) return aq_refuse("x265cu_aq_frame", bad);
+    cudaSetDevice(c->device);
+    const int L = p->qgSize == 8 ? 8 : 16;
+    const int nb = ((width + L - 1) / L) * ((height + L - 1) / L);
+    const int w8 = ((width / 2) + 7) >> 3, h8 = ((height / 2) + 7) >> 3;
+    const int blockCount = p->qgSize == 8 ? 4 * w8 * h8 : w8 * h8;
+    const size_t need = 6 * sizeof(uint64_t) + (size_t)nb * sizeof(uint32_t);
+    if (c->aq_bytes < need)
+    {
+        cudaFree(c->d_aq);
+        c->d_aq = NULL; c->aq_bytes = 0;
+        if (cudaMalloc(&c->d_aq, need) != cudaSuccess) { x265cu_set_error("x265cu_aq_frame: scratch", cudaGetLastError(), __FILE__, __LINE__); return -1; }
+        c->aq_bytes = need;
+    }
+    uint64_t* d_tot = (uint64_t*)c->d_aq;
+    uint32_t* d_energy = (uint32_t*)(d_tot + 6);
+    if (aq_energy_launch(c, depth, luma, stride, cb, cr, cstride, width, height, p->qgSize, d_energy, d_tot)) return -1;
+    std::vector<uint32_t> energy(nb);
+    uint64_t totals[6];
+    CU_CHECK(cudaMemcpyAsync(totals, d_tot, sizeof(totals), cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaMemcpyAsync(energy.data(), d_energy, (size_t)nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
+    x265cu_aq_out o = out ? *out : x265cu_aq_out{};
+    std::vector<int32_t> invq, invq8;
+    if (!o.invQscaleFactor) { invq.assign(blockCount, 0); o.invQscaleFactor = invq.data(); }       // Lowres::create zeroes it
+    if (p->qgSize == 8 && !o.invQscaleFactor8x8) { invq8.assign(w8 * h8, 0); o.invQscaleFactor8x8 = invq8.data(); }
+    aq_finish(depth, width, height, p, energy.data(), totals, &o);
+    if (p->aqMode != 0 && invQscale_dev)
+    {
+        const int32_t* src = p->qgSize == 8 ? o.invQscaleFactor8x8 : o.invQscaleFactor;
+        CU_CHECK(cudaMemcpyAsync(invQscale_dev, src, (size_t)w8 * h8 * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+        CU_CHECK(cudaStreamSynchronize(c->stream));
+    }
+    return 0;
 }

@@ -389,6 +389,33 @@ _AN_PROTOS["x265cu_lookahead_cost_batch"] = (I, [P, I, P, I, I, I, I, P])
 _AN_PROTOS["x265cu_lookahead_weights_analyse"] = (I, [P, I, P, P, P, I64, I, I, I, I64, P, P, P])
 _AN_PROTOS["x265cu_cutree"] = (I, [P, P, I, P, I, I, P, I])
 _AN_PROTOS["x265cu_cutree_estimates"] = (I, [P, I, P, P, I])
+
+
+# ---------------- adaptive quantisation (x265cu_aq_energy / x265cu_aq_finish / x265cu_aq_frame) ----------------
+class AqParams(C.Structure):
+    """x265cu_aq_params (include/x265_b200.h)"""
+    _fields_ = [("aqMode", C.c_int32), ("qgSize", C.c_int32), ("weightp", C.c_int32), ("variance", C.c_int32),
+                ("hevcAq", C.c_int32), ("hdr10Opt", C.c_int32), ("aqMotion", C.c_int32), ("reserved", C.c_int32),
+                ("aqStrength", C.c_double), ("quantOffsets", P)]
+
+
+class AqOut(C.Structure):
+    """x265cu_aq_out: host arrays, each may be NULL"""
+    _fields_ = [("qpAqOffset", P), ("invQscaleFactor", P), ("invQscaleFactor8x8", P), ("wp_sum", P), ("wp_ssd", P),
+                ("blockVariance", P), ("frameVariance", P)]
+
+
+def aq_geometry(W, H, qg_size):
+    """(energy grid blocks, blockCount, w8 * h8): the lengths of x265cu_aq_energy's energies, of qpAqOffset /
+    invQscaleFactor / blockVariance / quantOffsets, and of invQscaleFactor8x8."""
+    L = 8 if qg_size == 8 else 16
+    w8, h8 = ((W // 2) + 7) >> 3, ((H // 2) + 7) >> 3
+    return ((W + L - 1) // L) * ((H + L - 1) // L), (4 if qg_size == 8 else 1) * w8 * h8, w8 * h8
+
+
+_AN_PROTOS["x265cu_aq_energy"] = (I, [P, I, P, I, P, P, I, I, I, I, P, P])
+_AN_PROTOS["x265cu_aq_finish"] = (I, [I, I, I, C.POINTER(AqParams), P, P, C.POINTER(AqOut)])
+_AN_PROTOS["x265cu_aq_frame"] = (I, [P, I, P, I, P, P, I, I, I, C.POINTER(AqParams), P, C.POINTER(AqOut)])
 _PROTOS.update(_AN_PROTOS)
 
 

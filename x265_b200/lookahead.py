@@ -93,6 +93,7 @@ class Lookahead:
                                 has_planes=False, has_intra=False, invq=None))
         self.tab = lib.to_device(lib.mvcost_table(LOOKAHEAD_LAMBDA[depth], MVRANGE))
         self._full = None
+        self._chroma = None              # init_frame(aq=...): the staged 4:2:0 chroma pair
         self._pool = {}                  # size -> free device buffers: the per-step result / motion-field buffers are recycled
         lib.sync()                       # (a window's step made ~2000 cudaMalloc / cudaFree calls before: most of its host time)
 
@@ -104,9 +105,15 @@ class Lookahead:
         self._pool.setdefault(buf.nbytes, []).append(buf)
 
     # ---- Lowres::init: full-res luma (host) -> 4 half-pel planes with extended borders (device) ----
-    def init_frame(self, i, img, sync=True):
+    def init_frame(self, i, img, sync=True, *, cb=None, cr=None, aq=None):
         """Lowres::init of frame i from its full-resolution luma (host array, ideally pinned): strided H2D straight into the
-        PicYuv-like padded device plane, border extension (pixel.cpp:1027-1041) and the lowres kernel on the device."""
+        PicYuv-like padded device plane, border extension (pixel.cpp:1027-1041) and the lowres kernel on the device.
+
+        aq: None (the frame's invQscale comes from set_invqscale, if at all), or a dict of calcAdaptiveQuantFrame's
+        parameters: mode (rc.aqMode 0-3), strength, qg_size, weightp, variance, quant_offsets (blockCount floats or None).
+        Then the 4:2:0 chroma planes cb / cr (host, W / 2 x H / 2; None for 4:0:0) are staged next to the luma, the AQ pass
+        runs on the device and its host finish leaves the frame's invQscale resident (invQscaleFactor8x8 at qg_size 8), and
+        the frame record keeps qpAqOffset, wp_sum and wp_ssd (and blockVariance / frameVariance with variance)."""
         cu = self.cu
         img = np.ascontiguousarray(img)
         H, W = img.shape
@@ -121,9 +128,48 @@ class Lookahead:
         f = self.fr[i]
         cu.check(cu.L.x265cu_frame_init_lowres(cu.ctx, self.depth, self._full.ptr + forg, fs,
                                                *[p.ptr + self.lorg for p in f["planes"]], self.ls, self.w8 * 8, self.h8 * 8, MARGIN_X, MARGIN_Y))
+        if aq is not None:
+            self._aq_frame(i, self._full.ptr + forg, fs, W, H, cb, cr, aq)
         if sync:
             cu.sync()          # the host image may be released / the staging plane re-used
         f["has_planes"] = True
+
+    def _aq_frame(self, i, luma, fs, W, H, cb, cr, aq):
+        """calcAdaptiveQuantFrame of frame i through x265cu_aq_frame, on the staged planes."""
+        import ctypes as C
+        from .lib import AqParams, AqOut, aq_geometry
+        cu = self.cu
+        assert (cb is None) == (cr is None), "give both chroma planes or neither"
+        cw, chh = W // 2, H // 2
+        cptr = [None, None]
+        if cb is not None:
+            if self._chroma is None:
+                self._chroma = [cu.alloc(cw * chh * self.es) for _ in range(2)]
+            for k, pl in enumerate((cb, cr)):
+                pl = np.ascontiguousarray(pl)
+                assert pl.shape == (chh, cw)
+                cu.check(cu.L.x265cu_copy2d(cu.ctx, self._chroma[k].ptr, cw * self.es, pl.ctypes.data, cw * self.es, cw * self.es, chh, 0))
+                cptr[k] = self._chroma[k].ptr
+        qg = int(aq.get("qg_size", 32))
+        _, count, _ = aq_geometry(W, H, qg)
+        qo = aq.get("quant_offsets")
+        qo = None if qo is None else np.ascontiguousarray(qo, np.float32)
+        assert qo is None or qo.size == count
+        prm = AqParams(aqMode=int(aq.get("mode", 2)), qgSize=qg, weightp=int(bool(aq.get("weightp", False))),
+                       variance=int(bool(aq.get("variance", False))), aqStrength=float(aq.get("strength", 1.0)),
+                       quantOffsets=qo.ctypes.data if qo is not None else None)
+        f = self.fr[i]
+        rec = dict(qpAqOffset=np.zeros(count), wp_sum=np.zeros(3, np.uint64), wp_ssd=np.zeros(3, np.uint64))
+        if prm.variance:
+            rec.update(blockVariance=np.zeros(count, np.uint32), frameVariance=np.zeros(1))
+        out = AqOut(**{k: v.ctypes.data for k, v in rec.items()})
+        if prm.aqMode != 0 and f["invq"] is None:
+            f["invq"] = cu.alloc(4 * self.ncu)
+        cu.check(cu.L.x265cu_aq_frame(cu.ctx, self.depth, luma, fs, cptr[0], cptr[1], cw, W, H, C.byref(prm),
+                                      f["invq"].ptr if prm.aqMode != 0 else None, C.byref(out)))
+        if prm.variance:
+            rec["frameVariance"] = float(rec["frameVariance"][0])
+        f.update(rec)
 
     def set_invqscale(self, i, invq):
         """Lowres::invQscaleFactor of frame i (int32 per lowres CU, 256 = 1.0): the adaptive-quantisation weights that
@@ -280,6 +326,9 @@ class Lookahead:
         self.tab.free()
         if self._full is not None:
             self._full.free()
+        for b in self._chroma or []:
+            b.free()
+        self._chroma = None
         for free in self._pool.values():
             for b in free:
                 b.free()
