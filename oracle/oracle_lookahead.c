@@ -10,6 +10,7 @@
 #include "oracle.h"
 #include <string.h>
 #include <math.h>
+#include <limits.h>
 
 #define COST_MAX (1 << 28)               /* motion.h:65 */
 #define LOWRES_COST_MASK ((1 << 14) - 1) /* slicetype.h:41-42 */
@@ -227,6 +228,13 @@ void orc_lookahead_frame_cost(orc_la_job* j)
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct { int wtPresent, inputWeight, log2WeightDenom, inputOffset; } orc_wp;
 
+/* (int) of a float with x86 cvttss2si semantics (NaN and out-of-range values -> INT_MIN), which the reference's casts get
+ * from the compiler: on a fade from black refMean == 0 and the clamped offset's rescale divides by zero (slicetype.cpp:921). */
+static int la_cvttss2si(float v)
+{
+    return (v >= -2147483648.f && v < 2147483648.f) ? (int)v : INT_MIN;
+}
+
 static uint32_t la_weight_cost_luma(const pixel* fencBuf, const pixel* const* refBuf, pixel* wbuf, intptr_t stride, int width, int lines,
                                     int paddedLines, intptr_t padoffset, const int32_t* intraCost, const orc_wp* wp)
 {
@@ -272,7 +280,7 @@ int orc_la_weights_analyse(const pixel* fencBuf, const pixel* const* refBuf, pix
     unsigned int minscore = 0, origscore = 1;
     int found = 0;
     /* wp.setFromWeightAndOffset((int)(guessScale * 128 + 0.5f), 0, 7, true): note wtPresent stays 0 for the first cost */
-    wp.inputOffset = 0; wp.log2WeightDenom = 7; wp.inputWeight = (int)(guessScale * 128 + 0.5f);
+    wp.inputOffset = 0; wp.log2WeightDenom = 7; wp.inputWeight = la_cvttss2si(guessScale * 128 + 0.5f);
     while (wp.log2WeightDenom > 0 && wp.inputWeight > 127) { wp.log2WeightDenom--; wp.inputWeight >>= 1; }
     if (wp.inputWeight > 127) wp.inputWeight = 127;
     mindenom = wp.log2WeightDenom;
@@ -284,11 +292,11 @@ int orc_la_weights_analyse(const pixel* fencBuf, const pixel* const* refBuf, pix
 
     unsigned int s = 0;
     int curScale = minscale;
-    int curOffset = (int)(fencMean - refMean * curScale / (1 << mindenom) + 0.5f);
+    int curOffset = la_cvttss2si(fencMean - refMean * curScale / (1 << mindenom) + 0.5f);
     if (curOffset < -128 || curOffset > 127)
     {
         curOffset = curOffset < -128 ? -128 : (curOffset > 127 ? 127 : curOffset);
-        curScale = (int)((1 << mindenom) * (fencMean - curOffset) / refMean + 0.5f);
+        curScale = la_cvttss2si((1 << mindenom) * (fencMean - curOffset) / refMean + 0.5f);
         curScale = curScale < 0 ? 0 : (curScale > 127 ? 127 : curScale);
     }
     wp.inputWeight = curScale; wp.log2WeightDenom = mindenom; wp.inputOffset = curOffset; wp.wtPresent = 1;

@@ -6,9 +6,55 @@ import ctypes as C
 import numpy as np
 
 from common import P, I, IP, ptr, pixel_dtype
-from frame_helpers import pad_plane, MARGIN_X, MARGIN_Y, MVRANGE
+from frame_helpers import gen_luma, gen_chroma, pad_plane, MARGIN_X, MARGIN_Y, MVRANGE
 
 LOOKAHEAD_LAMBDA = {8: 1.0, 10: 16.0}     # x265_lambda_tab[X265_LOOKAHEAD_QP = 12 + 6*(depth-8)] (constants.cpp:33-130)
+
+# content_frames kinds, and what each one makes the lookahead do that the moving clip does not
+CONTENT_KINDS = ("static", "black", "white", "flat", "fast", "cut", "fade", "full10")
+FAST_MOTION = (44, -30)                   # px per frame: 22 / 15 lowres px, past the +-16 search range at every distance
+CUT_SEED = 9001
+
+
+def content_frames(kind, W, H, depth, n, plane=0):
+    """n frames of lookahead content `kind`: luma (plane 0) or the 4:2:0 Cb / Cr plane (1 / 2) of the same pictures.
+      static  one picture of the clip, repeated: every vector is (0, 0) and bidir ties list 0 (the zero-MV skip, the tie);
+      black / white  constant 0 / maxv: every intra mode and every vector cost the same;
+      flat    the clip with static letterbox bars and constant rectangles (frame_helpers._flat_areas);
+      fast    the clip moving FAST_MOTION px per frame: vectors end on their CU's search bound, predictors lie far away;
+      cut     the clip for the first n // 2 frames, then noise of another seed: the estimates across the cut go intra;
+      fade    the clip scaled from black up and back down to black (frames 0 and n - 1 are black);
+      full10  (10 bit) the clip over the whole 10-bit range, saturated at 0 and 1023."""
+    assert kind in CONTENT_KINDS and (kind != "full10" or depth == 10), (kind, depth)
+    if plane:
+        gen = lambda i, **kw: gen_chroma(W, H, i, plane, bits=depth, **kw)
+        shape = (H // 2, W // 2)
+    else:
+        gen = lambda i, **kw: gen_luma(W, H, i, bits=depth, **kw)
+        shape = (H, W)
+    if kind == "static":
+        f = gen(0)
+        return [f.copy() for _ in range(n)]
+    if kind in ("black", "white"):
+        return [np.full(shape, 0 if kind == "black" else (1 << depth) - 1, pixel_dtype(depth)) for _ in range(n)]
+    if kind == "flat":
+        return [gen(i, content="flat") for i in range(n)]
+    if kind == "fast":
+        return [gen(i, motion=FAST_MOTION) for i in range(n)]
+    if kind == "cut":
+        return [gen(i) if i < n // 2 else gen(i, seed=CUT_SEED, noise=True) for i in range(n)]
+    if kind == "fade":
+        half = (n - 1) / 2
+        return [np.rint(gen(i).astype(np.float64) * min(min(i, n - 1 - i) / half, 1.0)).astype(pixel_dtype(depth)) for i in range(n)]
+    return [gen(i, content="full10") for i in range(n)]
+
+
+def search_bounds(w8, h8):
+    """Per lowres CU, the qpel bounds (x min, x max, y min, y max) of its search: 8 px past the picture on every side
+    (estimateCUCost, slicetype.cpp:3248-3251).  Vectors lie inside them, inclusive."""
+    cx = np.arange(w8 * h8) % w8
+    cy = np.arange(w8 * h8) // w8
+    return 4 * (-cx * 8 - 8), 4 * ((w8 - cx - 1) * 8 + 8), 4 * (-cy * 8 - 8), 4 * ((h8 - cy - 1) * 8 + 8)
 
 
 class OrcLaJob(C.Structure):

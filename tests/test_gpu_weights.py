@@ -9,9 +9,9 @@ import numpy as np
 import pytest
 
 from common import load_oracle, ptr, P, I, IP, pixel_dtype
-from frame_helpers import gen_luma, MARGIN_X, MARGIN_Y
+from frame_helpers import MARGIN_X, MARGIN_Y
 from lookahead_helpers import OracleLookahead
-from test_lookahead_oracle_vs_ref import _wp_stats
+from test_lookahead_oracle_vs_ref import _wp_stats, weights_decision, weights_frames
 
 pytestmark = pytest.mark.gpu
 
@@ -24,16 +24,10 @@ def cu():
 
 @pytest.mark.timeout(180)
 @pytest.mark.parametrize("depth", [8, 10])
-@pytest.mark.parametrize("case", ["same", "fade", "fade2", "bright", "offset"])
+@pytest.mark.parametrize("case", ["same", "fade", "fade2", "bright", "offset", "from_black_dark", "from_black_bright", "to_black", "constant"])
 def test_weights_analyse(cu, depth, case):
     O = load_oracle(depth)
-    W, H = 416, 240
-    mx = (1 << depth) - 1
-    sc = 1 << (depth - 8)
-    base = gen_luma(W, H, 0, s1=17.0, s2=11.0, bits=depth).astype(np.float64)
-    nxt = gen_luma(W, H, 1, s1=17.0, s2=11.0, bits=depth).astype(np.float64)
-    cur = {"same": nxt, "fade": nxt * 0.78, "fade2": nxt * 0.55 + 1 * sc, "bright": nxt * 1.07, "offset": nxt + 21 * sc}[case]
-    frames = [base.astype(pixel_dtype(depth)), np.clip(np.rint(cur), 0, mx).astype(pixel_dtype(depth))]
+    frames = weights_frames(case, depth)
     orc = OracleLookahead(O, frames, depth)
     planes = [orc.fr[f]["planes"] for f in range(2)]                   # whole padded buffers (Lowres::buffer[i])
     rows, stride = planes[0][0].shape
@@ -49,7 +43,7 @@ def test_weights_analyse(cu, depth, case):
     O.orc_la_weights_analyse.argtypes = [P, P, P, IP, IP, I, I, IP, P, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, P]
     want = O.orc_la_weights_analyse(ptr(planes[1][0]), refarr, ptr(worc), planesize, stride, lw, lh, padoffset, ptr(intra),
                                     int(stats[0]), int(stats[1]), int(stats[2]), int(stats[3]), ptr(wp))
-    assert (want == 0) == (case in ("same", "offset"))
+    assert want == weights_decision(case)
 
     d_fenc = cu.to_device(planes[1][0])
     d_refs = [cu.to_device(p) for p in planes[0]]

@@ -9,7 +9,7 @@ import pytest
 
 from common import load_ref, load_oracle, ptr, P, I, IP, pixel_dtype
 from frame_helpers import gen_luma, MARGIN_X, MARGIN_Y
-from lookahead_helpers import OracleLookahead
+from lookahead_helpers import OracleLookahead, CONTENT_KINDS, content_frames, lowres_geometry, search_bounds
 from ref_results import RefResults
 
 TRIPLES = [(0, 1, 1), (0, 2, 1), (0, 2, 2), (0, 3, 1), (0, 3, 2), (0, 3, 3), (1, 3, 2), (2, 3, 3)]
@@ -68,6 +68,12 @@ def test_lookahead(depth, size, noise, request):
     frames = [gen_luma(W, H, i, s1=17.0, s2=11.0, bits=depth, noise=noise) for i in range(4)]
     ref = RefLookahead(G.R, frames) if G.R else None
     orc = OracleLookahead(O, frames, depth)
+    _same_estimates(G, ref, orc, depth, TRIPLES)
+
+
+def _same_estimates(G, ref, orc, depth, triples):
+    """Lowres planes of frame 1, every frame's intra estimate, and per triple the frame cost, per-CU costs, row sums, motion
+    fields (list 0 vectors and costs, list 1 vectors) and costEst / costEstAq / intraMbs of the oracle against the reference."""
     G.same("geometry", lambda: (ref.w8, ref.h8, ref.stride), (orc.w8, orc.h8, orc.stride))
     # lowres planes incl. margins (Lowres::init)
     lw, lh = [int(x) for x in G.value("lowres_size", lambda: (ref.lw, ref.lh))]
@@ -75,12 +81,12 @@ def test_lookahead(depth, size, noise, request):
     for k in range(4):
         G.same("plane%d" % k, lambda: ref.get(1, 7, k, 0, pixel_dtype(depth), rows * ref.stride).reshape(rows, ref.stride)[:, :vw],
                orc.fr[1]["planes"][k][:, :vw])
-    for f in range(4):
+    for f in range(len(orc.fr)):
         G.same("intraCost%d" % f, lambda: ref.get(f, 0), orc.fr[f]["intraCost"])
         G.same("intraMode%d" % f, lambda: ref.get(f, 1, dtype=np.uint8), orc.fr[f]["intraMode"])
         G.same("lowresCosts%d" % f, lambda: ref.get(f, 2, 0, 0, np.uint16), orc.fr[f]["lowresCosts"][(0, 0)])
         G.same("rowSatds%d" % f, lambda: ref.get(f, 3, 0, 0, np.int32, ref.h8), orc.fr[f]["rowSatds"][(0, 0)])
-    for (p0, p1, b) in TRIPLES:
+    for (p0, p1, b) in triples:
         t = "%d%d%d" % (p0, p1, b)
         c = orc.cost(p0, p1, b)
         G.same("cost" + t, lambda: ref.cost(p0, p1, b), c)
@@ -133,6 +139,127 @@ def _cooperative_slices(request, depth, lslices, W, H):
                for t in [(0, 1, 1), (0, 2, 2)])
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# the lookahead on content other than the moving clip (lookahead_helpers.content_frames): static and constant pictures,
+# static flat areas, motion past the search range, a cut to noise, fades through black, the full 10-bit range
+CONTENT_CASES = [(k, d) for k in CONTENT_KINDS for d in (8, 10) if k != "full10" or d == 10]
+CONTENT_SIZES = [(416, 240), (200, 136)]               # 200x136: 100x68 lowres px, partial CUs on the right and at the bottom
+
+
+def searched_fields(orc):
+    """(frame, (list, distance), vectors, costs) of every motion field a triple searched (P triples also create the
+    list-1 field of distance 0, which nothing searches)."""
+    return [(b, k, f["mvs"][k], f["mvcosts"][k]) for b, f in enumerate(orc.fr) for k in f["mvs"] if k[1] > 0]
+
+
+def assert_content_reaches(kind, depth, orc, triples):
+    """What each kind is there for, asserted on the oracle's outputs, so that no case quietly stops reaching it."""
+    fields = searched_fields(orc)
+    if kind in ("static", "black", "white", "flat"):
+        # the bidir zero-MV skip: the search result (which includes a vector cost) replaced by the bare SATD at (0, 0)
+        assert any(((c == 0) & (m == 0).all(axis=1)).any() for _, _, m, c in fields), "no zero-MV skip"
+    if kind in ("black", "white"):
+        modes = np.concatenate([f["intraMode"] for f in orc.fr])
+        assert (modes == modes[0]).all(), "a constant picture must leave a single intra mode (all 35 tie)"
+    if kind == "fast":
+        lx, hx, ly, hy = search_bounds(orc.w8, orc.h8)
+        assert any(((m[:, 0] == lx) | (m[:, 0] == hx) | (m[:, 1] == ly) | (m[:, 1] == hy)).any() for _, _, m, _ in fields), \
+            "no vector on its CU's search bound"
+    if kind == "cut":
+        n = len(orc.fr)
+        across = [(p0, b) for (p0, p1, b) in triples if p1 == b and p0 < n // 2 <= b]
+        assert across and all(orc.fr[b]["estIntraMbs"][(b - p0, 0)] > 0 for p0, b in across), "no intra CU across the cut"
+        if depth == 10:
+            assert any(((v & 0x3FFF) == 0x3FFF).any() for f in orc.fr for v in f["lowresCosts"].values()), \
+                "10-bit noise must saturate a per-CU cost at LOWRES_COST_MASK"
+    if kind == "fade":
+        assert orc.fr[1]["estIntraMbs"][(1, 0)] > 0, "the P estimate from the black frame has no intra CU"
+
+
+@pytest.mark.parametrize("size", CONTENT_SIZES, ids=["%dx%d" % s for s in CONTENT_SIZES])
+@pytest.mark.parametrize("kind,depth", CONTENT_CASES)
+def test_lookahead_content(kind, depth, size, request):
+    """The comparisons of test_lookahead, plus every frame's lowres planes and the list-1 vector costs, on each kind of
+    content_frames: the zero-MV skip and the bidir tie (static, constant, flat), the full-tie intra search (constant),
+    vectors on the search bounds and far predictors (fast), intra CUs and saturated costs (cut, fade), the full 10-bit
+    range (full10)."""
+    G = RefResults(request, depth)
+    O = load_oracle(depth)
+    W, H = size
+    frames = content_frames(kind, W, H, depth, 4)
+    ref = RefLookahead(G.R, frames) if G.R else None
+    orc = OracleLookahead(O, frames, depth)
+    _same_estimates(G, ref, orc, depth, TRIPLES)
+    _same_planes_and_list1_costs(G, ref, orc, depth, TRIPLES)
+    assert_content_reaches(kind, depth, orc, TRIPLES)
+
+
+def _same_planes_and_list1_costs(G, ref, orc, depth, triples):
+    lw, lh = [int(x) for x in G.value("lowres_size", lambda: (ref.lw, ref.lh))]
+    rows, vw = lh + 2 * MARGIN_Y, lw + 2 * MARGIN_X
+    for f in range(len(orc.fr)):
+        G.same("planes%d" % f, lambda: [ref.get(f, 7, k, 0, pixel_dtype(depth), rows * ref.stride).reshape(rows, ref.stride)[:, :vw]
+                                        for k in range(4)], [orc.fr[f]["planes"][k][:, :vw] for k in range(4)])
+    for (p0, p1, b) in triples:
+        if p1 > b:
+            G.same("mvcosts1%d%d%d" % (p0, p1, b), lambda: ref.get(b, 5, 1, p1 - b), orc.fr[b]["mvcosts"][(1, p1 - b)])
+
+
+@pytest.mark.parametrize("lslices", [4, 8])
+@pytest.mark.parametrize("kind", ["static", "fast"])
+def test_lookahead_content_cooperative_slices(kind, lslices, request):
+    """Cooperative slices at 1280x720 on static content (every slice's bottom row loses its predictors from below, which
+    are all (0, 0) anyway) and on fast motion (each slice's bottom row then searches from the right neighbour alone)."""
+    depth, W, H = 8, 1280, 720
+    G = RefResults(request, depth)
+    O = load_oracle(depth)
+    frames = content_frames(kind, W, H, depth, 3)
+    triples = [(0, 1, 1), (0, 2, 1), (0, 2, 2)]
+    ref = RefLookahead(G.R, frames, lslices=lslices) if G.R else None
+    slices = tuple(int(x) for x in G.value("slices", lambda: ref.slices))
+    assert slices[0] > 1, slices
+    orc = OracleLookahead(O, frames, depth, slices=slices)
+    _same_estimates(G, ref, orc, depth, triples)
+    assert_content_reaches(kind, depth, orc, triples)
+    if kind == "fast":
+        ser = OracleLookahead(O, frames, depth)
+        for t in triples:
+            ser.cost(*t)
+        assert any(not np.array_equal(ser.fr[b]["mvs"][(0, b - p0)], orc.fr[b]["mvs"][(0, b - p0)]) for (p0, p1, b) in triples), \
+            "the slices do not change the motion fields"
+
+
+# (aqMode, strength, qgSize, weightp, variance, quantOffsets) of x265ref_la_create_aq: AUTO_VARIANCE, strength 1.0, qgSize 32
+AQ_PARAMS = (2, 1.0, 32, 0, 0, 0)
+
+
+def content_invq(kind, W, H, depth, frames):
+    """Lowres::invQscaleFactor of every frame from the AQ restatement (aq_helpers.oracle), with chroma of the same kind."""
+    import aq_helpers as A
+    chroma = [(c1, c2) for c1, c2 in zip(content_frames(kind, W, H, depth, len(frames), 1), content_frames(kind, W, H, depth, len(frames), 2))]
+    invq = [A.oracle((y, cb, cr), W, H, depth, AQ_PARAMS)["invQscaleFactor"].astype(np.int32) for y, (cb, cr) in zip(frames, chroma)]
+    return chroma, invq
+
+
+@pytest.mark.parametrize("depth", [8, 10])
+@pytest.mark.parametrize("kind", ["flat", "static", "cut"])
+def test_lookahead_content_with_adaptive_quant(kind, depth, request):
+    """Adaptive quantisation on flat areas (zero-energy blocks), static and cut content: the AQ restatement's
+    invQscaleFactor equals the real calcAdaptiveQuantFrame's, and with it every estimate equals the reference's."""
+    G = RefResults(request, depth)
+    O = load_oracle(depth)
+    W, H = 416, 240
+    frames = content_frames(kind, W, H, depth, 4)
+    chroma, invq = content_invq(kind, W, H, depth, frames)
+    assert any((q != 256).any() for q in invq), "AQ produced no offsets: the test would not see invQscale"
+    ref = RefLookahead(G.R, frames, aq=2, chroma=chroma) if G.R else None
+    for i in range(len(frames)):
+        G.same("invq%d" % i, lambda: ref.get(i, 8), invq[i])
+    orc = OracleLookahead(O, frames, depth, invq=invq)
+    _same_estimates(G, ref, orc, depth, TRIPLES)
+    assert_content_reaches(kind, depth, orc, TRIPLES)
+
+
 def aq_inputs(request, depth, lslices, W=1280, H=720):
     """Frames of the AQ cases and the reference's (numCoopSlices, numRowsPerSlice) and per-frame Lowres::invQscaleFactor,
     which the code under test takes as inputs (there is no restatement of calcAdaptiveQuantFrame)."""
@@ -180,23 +307,59 @@ def _wp_stats(img):
     return s, q - (s * s + n // 2) // n
 
 
+# (reference, current) pictures of the weights analysis: fades that take every exit of the analysis
+WEIGHTS_CASES = ["same", "fade", "fade2", "bright", "offset", "noise_fade", "from_black_dark", "from_black_bright", "to_black", "constant"]
+
+
+def weights_frames(case, depth, W=416, H=240):
+    """The two luma pictures of a WEIGHTS_CASES case.  NB the analysis estimates means from full-resolution sums over the
+    LOWRES area (slicetype.cpp:892-893), i.e. 4x the true means, so only (nearly) pure scalings end up weighted; "offset"
+    takes the rejected path.  The fades from black have a reference with wp_sum == wp_ssd == 0: the dark one (4x mean below
+    127.5) keeps its offset, the bright one clamps it to 127 and divides by refMean == 0 (slicetype.cpp:921)."""
+    mx = (1 << depth) - 1
+    sc = 1 << (depth - 8)
+    base = gen_luma(W, H, 0, s1=17.0, s2=11.0, bits=depth, noise=case.startswith("noise")).astype(np.float64)
+    nxt = gen_luma(W, H, 1, s1=17.0, s2=11.0, bits=depth, noise=case.startswith("noise")).astype(np.float64)
+    black = np.zeros_like(base)
+    ref, cur = {"from_black_dark": (black, nxt * 0.15), "from_black_bright": (black, nxt * 0.6), "to_black": (base, black),
+                "constant": (black + 60 * sc, black + 150 * sc)}.get(case, (base, None))
+    if cur is None:
+        cur = {"same": nxt, "fade": nxt * 0.78, "fade2": nxt * 0.55 + 1 * sc, "bright": nxt * 1.07, "offset": nxt + 21 * sc,
+               "noise_fade": nxt * 0.6}[case]
+    return [np.clip(np.rint(f), 0, mx).astype(pixel_dtype(depth)) for f in (ref, cur)]
+
+
+def weights_offset_clamped(frames, depth):
+    """Whether the analysis of `frames` clamps its first offset guess (slicetype.cpp:914-915), in the float arithmetic of
+    the analysis: the curScale that follows divides by refMean."""
+    f32 = np.float32
+    lw, lh = [8 * g for g in lowres_geometry(*frames[0].shape[::-1])[:2]]
+    (fs, fq), (rs, rq) = _wp_stats(frames[1]), _wp_stats(frames[0])
+    fencMean = f32(f32(fs) / f32(lw * lh)) / f32(1 << (depth - 8))
+    refMean = f32(f32(rs) / f32(lw * lh)) / f32(1 << (depth - 8))
+    guess = np.sqrt(f32(fq) / f32(rq)) if fq and rq else f32(1.0)
+    scale, denom = int(guess * f32(128) + f32(0.5)), 7
+    while denom > 0 and scale > 127:
+        denom, scale = denom - 1, scale >> 1
+    off = int(fencMean - refMean * f32(min(scale, 127)) / f32(1 << denom) + f32(0.5))
+    return not -128 <= off <= 127, float(refMean)
+
+
+def weights_decision(case):
+    """Lowres::weightedRef[].isWeighted of a case.  Not weighted: "same" and "offset" (no gain), noise (inter never beats
+    intra), the fades from black (a constant reference never beats intra) and the constant pair (every CU is intra either
+    way).  The fade to black ends weighted: scale 1/4, offset -128."""
+    return int(case in ("fade", "fade2", "bright", "to_black"))
+
+
 @pytest.mark.parametrize("depth", [8, 10])
-@pytest.mark.parametrize("case", ["same", "fade", "fade2", "bright", "offset", "noise_fade"])
+@pytest.mark.parametrize("case", WEIGHTS_CASES)
 def test_lookahead_weights_analyse(depth, case, request):
     """LookaheadTLD::weightsAnalyse + weightCostLuma (slicetype.cpp:807-961): the decision and the 4 re-weighted lowres
     planes of the oracle against the real class, on fades that take every exit of the analysis."""
     G = RefResults(request, depth)
     O = load_oracle(depth)
-    W, H = 416, 240
-    mx = (1 << depth) - 1
-    base = gen_luma(W, H, 0, s1=17.0, s2=11.0, bits=depth, noise=case.startswith("noise")).astype(np.float64)
-    nxt = gen_luma(W, H, 1, s1=17.0, s2=11.0, bits=depth, noise=case.startswith("noise")).astype(np.float64)
-    sc = 1 << (depth - 8)
-    # NB the analysis estimates the offset from full-resolution sums over the LOWRES area (slicetype.cpp:892-893), i.e. 4x the
-    # true mean difference, so only (nearly) pure scalings end up weighted; "offset" exercises the rejected path
-    cur = {"same": nxt, "fade": nxt * 0.78, "fade2": nxt * 0.55 + 1 * sc, "bright": nxt * 1.07, "offset": nxt + 21 * sc,
-           "noise_fade": nxt * 0.6}[case]
-    frames = [base.astype(pixel_dtype(depth)), np.clip(np.rint(cur), 0, mx).astype(pixel_dtype(depth))]
+    frames = weights_frames(case, depth)
     ref = RefLookahead(G.R, frames) if G.R else None
     orc = OracleLookahead(O, frames, depth)
     lw, lh = [int(x) for x in G.value("lowres_size", lambda: (ref.lw, ref.lh))]
@@ -225,6 +388,8 @@ def test_lookahead_weights_analyse(depth, case, request):
                                      MARGIN_Y * orc.stride + MARGIN_X, ptr(intra),
                                      int(stats[0]), int(stats[1]), int(stats[2]), int(stats[3]), ptr(wp))
     G.same("weights", ref_weights, [got_o, worc if got_o else 0])
-    assert (got_o == 0) == (case in ("same", "offset", "noise_fade")), (case, got_o)   # noise: inter never beats intra, no gain
+    assert got_o == weights_decision(case), (case, got_o)
+    if case.startswith("from_black"):
+        assert weights_offset_clamped(frames, depth) == (case == "from_black_bright", 0.0), case
     if got_o:
         assert 0 <= wp[0] <= 127 and 0 <= wp[1] <= 7 and -128 <= wp[2] <= 127

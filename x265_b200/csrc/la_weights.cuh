@@ -9,11 +9,20 @@
 #include "common.cuh"
 #include "blockops.cuh"
 #include "pixelcmp_grid.cuh"
+#include <limits.h>
 #include <math.h>
 
 namespace law {
 
 struct Wp { int wtPresent, inputWeight, log2WeightDenom, inputOffset; };
+
+// (int) of a float as x86's cvttss2si computes it: NaN and values outside the int range give INT_MIN.  C leaves those
+// conversions undefined, and the analysis makes one on a fade from black: refMean == 0 with the offset clamped divides
+// by zero (slicetype.cpp:921), and curScale then clamps +inf's INT_MIN to 0.
+static inline int la_cvttss2si(float v)
+{
+    return (v >= -2147483648.f && v < 2147483648.f) ? (int)v : INT_MIN;
+}
 
 struct Run
 {
@@ -128,7 +137,7 @@ extern "C" int x265cu_lookahead_weights_analyse(x265cu_ctx* c, int depth, const 
     int found = 0;
     Wp wp = { 0, 0, 0, 0 };
     /* wp.setFromWeightAndOffset((int)(guessScale * 128 + 0.5f), 0, 7, true) (slice.h:304-316); wtPresent stays 0 */
-    wp.inputOffset = 0; wp.log2WeightDenom = 7; wp.inputWeight = (int)(guessScale * 128 + 0.5f);
+    wp.inputOffset = 0; wp.log2WeightDenom = 7; wp.inputWeight = la_cvttss2si(guessScale * 128 + 0.5f);
     while (wp.log2WeightDenom > 0 && wp.inputWeight > 127) { wp.log2WeightDenom--; wp.inputWeight >>= 1; }
     if (wp.inputWeight > 127) wp.inputWeight = 127;
     mindenom = wp.log2WeightDenom;
@@ -141,11 +150,11 @@ extern "C" int x265cu_lookahead_weights_analyse(x265cu_ctx* c, int depth, const 
         return 0;
 
     int curScale = minscale;
-    int curOffset = (int)(fencMean - refMean * curScale / (1 << mindenom) + 0.5f);
+    int curOffset = la_cvttss2si(fencMean - refMean * curScale / (1 << mindenom) + 0.5f);
     if (curOffset < -128 || curOffset > 127)
     {
         curOffset = curOffset < -128 ? -128 : (curOffset > 127 ? 127 : curOffset);
-        curScale = (int)((1 << mindenom) * (fencMean - curOffset) / refMean + 0.5f);
+        curScale = la_cvttss2si((1 << mindenom) * (fencMean - curOffset) / refMean + 0.5f);
         curScale = curScale < 0 ? 0 : (curScale > 127 ? 127 : curScale);
     }
     wp.inputWeight = curScale; wp.log2WeightDenom = mindenom; wp.inputOffset = curOffset; wp.wtPresent = 1;
