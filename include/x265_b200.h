@@ -542,6 +542,62 @@ int x265cu_aq_finish(int depth, int width, int height, const x265cu_aq_params* p
 int x265cu_aq_frame(x265cu_ctx*, int depth, const void* luma, int stride, const void* cb, const void* cr, int cstride,
                     int width, int height, const x265cu_aq_params* params, int32_t* invQscale_dev, const x265cu_aq_out* out);
 
+/* Weighted-prediction analysis of a P / B slice: weightAnalyse (encoder/weightPrediction.cpp:222-539), the frame encoder's
+ * choice of the slice's pred_weight_table for luma and both chroma planes, on the lookahead's device-resident lowres
+ * planes, intra costs and motion fields and the source chroma.  The candidate costs (weightCost, :169-218, after mcLuma /
+ * mcChroma, :60-163) are k_weightp_costs on the device: one warp per 8x8 block, the motion-compensated reference block
+ * formed in shared memory (no weighted or compensated plane is written), every candidate scored from it with the
+ * reference's 8x4-tiled SATD and wrapping uint32 sums.  The search (:260-501) is a literal restatement on the host: its
+ * candidates depend on the picture statistics only, so one launch and one download per plane and list serve it.
+ * Refs 1..numRefIdx-1 of each list are reset as the reference resets them; entries past numRefIdx[list], and list 1 of
+ * a P slice, are left untouched (the reference never writes them).  8 and 10 bit; 4:2:0 and 4:0:0.  In 4:0:0 the
+ * reference picks the chroma denominator from two uninitialised floats (:280-286); here it stays 7. */
+typedef struct {
+    const void* lowres[4];      /* the 4 lowres hpel planes (Lowres::lowresPlane) at picture origin, margins extended */
+    const void* cb;             /* full-resolution source Cb / Cr at (0,0), margins extended; NULL for 4:0:0 */
+    const void* cr;
+    int32_t lowresStride, chromaStride;   /* in pixels */
+    uint64_t wp_sum[3], wp_ssd[3];        /* Lowres::wp_sum / wp_ssd, as calcAdaptiveQuantFrame leaves them */
+    int32_t poc, reserved;
+} x265cu_wp_frame;
+typedef struct {
+    int32_t sliceType;          /* 0 B (two lists), 1 P (list 0) */
+    int32_t numRefIdx[2];       /* Slice::m_numRefIdx, 1..16 for each list the slice uses */
+    int32_t bframes;            /* param.bframes: motion fields are used for diffPoc <= bframes + 1 */
+    int32_t width, height;      /* m_picWidth / m_picHeight, multiples of 8 */
+    int32_t csp;                /* 0 = 4:0:0, 1 = 4:2:0 */
+} x265cu_wp_params;
+typedef struct { int32_t weighted, w0, denom, offset; } x265cu_wp_cand;     /* weighted = 0: the unweighted reference */
+typedef struct { int32_t wtPresent, inputWeight, log2WeightDenom, inputOffset; } x265cu_wp_entry;
+
+/* weightCost of each candidate for one plane (0 luma on the lowres planes, 1 Cb, 2 Cr) of fenc against ref, without the
+ * slice-header cost: costs[i] = sum over the 8x8 blocks of satd (luma: min(satd, intraCost[cu])) in wrapping uint32.  A
+ * weighted candidate weights each reference pixel as weight_pp does, offset = candidate offset << (depth - 8).
+ * mvs_dev: lowresMvs[list][diffPoc] as int32 pairs (w8 * h8, device) or NULL for no motion compensation.  intraCost_dev
+ * (w8 * h8, device) is read for luma.  Records are host structs holding device pointers.  Chroma motion compensation
+ * reads the reference chroma from column / row -9 to cw + 16 / ch + 16, where cw = ((width >> 4) << 4) >> 1 and
+ * ch = ((height >> 4) << 4) >> 1: the caller extends the borders at least that far (PicYuv's 48 x 40 chroma margins
+ * do); luma reads within 8 + 8 lowres pixels of the lowres picture.  1..48 candidates (w0 0..127, denom 0..7, offset
+ * -128..127).  Returns -1 before any launch (x265cu_last_error) on bad arguments.  Synchronises the context's stream. */
+int x265cu_weightp_costs(x265cu_ctx*, int depth, const x265cu_wp_params* params, const x265cu_wp_frame* fenc,
+                         const x265cu_wp_frame* ref, const int32_t* intraCost_dev, const int32_t* mvs_dev, int plane,
+                         const x265cu_wp_cand* cands, int ncand, uint32_t* costs);
+
+/* The cost provider of x265cu_weightp_decide: fill costs[0..n) for the candidates of (list, plane), with motion
+ * compensation when use_mvs.  Returns 0, or -1 to abort the decision. */
+typedef int (*x265cu_wp_cost_fn)(void* user, int list, int plane, int use_mvs, const x265cu_wp_cand* cands, int n,
+                                 uint32_t* costs);
+/* The search of weightAnalyse on costs from `cost` (needs no device).  fenc / refs[list] give poc and the picture
+ * statistics; has_mvs[list] says whether lowresMvs[list][diffPoc] was searched.  out: [2][16][3] entries. */
+int x265cu_weightp_decide(int depth, const x265cu_wp_params* params, const x265cu_wp_frame* fenc,
+                          const x265cu_wp_frame* const* refs, const int32_t* has_mvs, x265cu_wp_cost_fn cost, void* user,
+                          x265cu_wp_entry* out);
+/* The whole analysis on the device: refs[list] = m_refFrameList[list][0], mvs_dev[list] = lowresMvs[list][diffPoc]
+ * (NULL: not searched), intraCost_dev of fenc.  One cost launch and one download per analysed plane and list. */
+int x265cu_weightp_analyse(x265cu_ctx*, int depth, const x265cu_wp_params* params, const x265cu_wp_frame* fenc,
+                           const int32_t* intraCost_dev, const x265cu_wp_frame* const* refs, const int32_t* const* mvs_dev,
+                           x265cu_wp_entry* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -419,6 +419,40 @@ _AN_PROTOS["x265cu_aq_frame"] = (I, [P, I, P, I, P, P, I, I, I, C.POINTER(AqPara
 _PROTOS.update(_AN_PROTOS)
 
 
+# ---------------- weighted-prediction analysis (x265cu_weightp_costs / _decide / _analyse) ----------------
+class WpFrame(C.Structure):
+    """x265cu_wp_frame (include/x265_b200.h): device planes at picture origin, the picture statistics and the poc"""
+    _fields_ = [("lowres", P * 4), ("cb", P), ("cr", P), ("lowresStride", C.c_int32), ("chromaStride", C.c_int32),
+                ("wp_sum", C.c_uint64 * 3), ("wp_ssd", C.c_uint64 * 3), ("poc", C.c_int32), ("reserved", C.c_int32)]
+
+
+class WpParams(C.Structure):
+    """x265cu_wp_params: sliceType 0 B / 1 P, csp 0 4:0:0 / 1 4:2:0"""
+    _fields_ = [("sliceType", C.c_int32), ("numRefIdx", C.c_int32 * 2), ("bframes", C.c_int32), ("width", C.c_int32),
+                ("height", C.c_int32), ("csp", C.c_int32)]
+
+
+class WpCand(C.Structure):
+    _fields_ = [("weighted", C.c_int32), ("w0", C.c_int32), ("denom", C.c_int32), ("offset", C.c_int32)]
+
+
+class WpEntry(C.Structure):
+    _fields_ = [("wtPresent", C.c_int32), ("inputWeight", C.c_int32), ("log2WeightDenom", C.c_int32), ("inputOffset", C.c_int32)]
+
+
+WP_COST_FN = C.CFUNCTYPE(C.c_int, P, C.c_int, C.c_int, C.c_int, C.POINTER(WpCand), C.c_int, C.POINTER(C.c_uint32))
+
+_WP_PROTOS = {
+    "x265cu_weightp_costs": (I, [P, I, C.POINTER(WpParams), C.POINTER(WpFrame), C.POINTER(WpFrame), P, P, I,
+                                 C.POINTER(WpCand), I, P]),
+    "x265cu_weightp_decide": (I, [I, C.POINTER(WpParams), C.POINTER(WpFrame), C.POINTER(C.POINTER(WpFrame)), P,
+                                  WP_COST_FN, P, P]),
+    "x265cu_weightp_analyse": (I, [P, I, C.POINTER(WpParams), C.POINTER(WpFrame), P, C.POINTER(C.POINTER(WpFrame)),
+                                   C.POINTER(P), P]),
+}
+_PROTOS.update(_WP_PROTOS)
+
+
 class Analyser:
     """Host mirror of x265cu_analyser: the public call a user makes for one frame is analyse()."""
 

@@ -12,6 +12,7 @@ The 4 half-pel planes of every frame are produced on its owner and published wit
 import numpy as np
 
 MARGIN_X, MARGIN_Y = 96, 80               # Lowres / PicYuv luma margins (common/lowres.cpp:59-63, picyuv.cpp:87-88)
+CMARGIN_X, CMARGIN_Y = 48, 40             # PicYuv 4:2:0 chroma margins
 MVRANGE = 65536
 LOOKAHEAD_LAMBDA = {8: 1.0, 10: 16.0}     # x265_lambda_tab[X265_LOOKAHEAD_QP = 12 + 6*(depth-8)] (constants.cpp:33-130)
 
@@ -105,7 +106,7 @@ class Lookahead:
         self._pool.setdefault(buf.nbytes, []).append(buf)
 
     # ---- Lowres::init: full-res luma (host) -> 4 half-pel planes with extended borders (device) ----
-    def init_frame(self, i, img, sync=True, *, cb=None, cr=None, aq=None):
+    def init_frame(self, i, img, sync=True, *, cb=None, cr=None, aq=None, keep_chroma=False):
         """Lowres::init of frame i from its full-resolution luma (host array, ideally pinned): strided H2D straight into the
         PicYuv-like padded device plane, border extension (pixel.cpp:1027-1041) and the lowres kernel on the device.
 
@@ -113,7 +114,10 @@ class Lookahead:
         parameters: mode (rc.aqMode 0-3), strength, qg_size, weightp, variance, quant_offsets (blockCount floats or None).
         Then the 4:2:0 chroma planes cb / cr (host, W / 2 x H / 2; None for 4:0:0) are staged next to the luma, the AQ pass
         runs on the device and its host finish leaves the frame's invQscale resident (invQscaleFactor8x8 at qg_size 8), and
-        the frame record keeps qpAqOffset, wp_sum and wp_ssd (and blockVariance / frameVariance with variance)."""
+        the frame record keeps qpAqOffset, wp_sum and wp_ssd (and blockVariance / frameVariance with variance).
+
+        keep_chroma: keep cb / cr resident for this frame in PicYuv-like buffers (48 x 40 margins, borders extended), as
+        weight_analyse() reads them."""
         cu = self.cu
         img = np.ascontiguousarray(img)
         H, W = img.shape
@@ -130,6 +134,13 @@ class Lookahead:
                                                *[p.ptr + self.lorg for p in f["planes"]], self.ls, self.w8 * 8, self.h8 * 8, MARGIN_X, MARGIN_Y))
         if aq is not None:
             self._aq_frame(i, self._full.ptr + forg, fs, W, H, cb, cr, aq)
+        # weight_analyse reads only what this init_frame left: the statistics of its AQ pass and the chroma it kept
+        self.fr[i]["wp_valid"] = aq is not None
+        if keep_chroma:
+            self._keep_chroma(i, cb, cr)
+        else:
+            for buf in self.fr[i].pop("chroma", None) or []:      # a re-used slot must not keep the previous frame's chroma
+                buf.free()
         if sync:
             cu.sync()          # the host image may be released / the staging plane re-used
         f["has_planes"] = True
@@ -170,6 +181,67 @@ class Lookahead:
         if prm.variance:
             rec["frameVariance"] = float(rec["frameVariance"][0])
         f.update(rec)
+
+    def _keep_chroma(self, i, cb, cr):
+        """frame i's 4:2:0 chroma in its own padded buffers, borders extended (the reference's m_bChromaExtended)"""
+        cu = self.cu
+        cw, chh = self.W // 2, self.H // 2
+        cs = ((self.W + 63) // 64 * 64) // 2 + 2 * CMARGIN_X
+        rows = ((self.H + 63) // 64 * 64) // 2 + 2 * CMARGIN_Y
+        corg = (CMARGIN_Y * cs + CMARGIN_X) * self.es
+        f = self.fr[i]
+        if f.get("chroma") is None:
+            f["chroma"] = [cu.alloc(cs * rows * self.es) for _ in range(2)]
+        for buf, pl in zip(f["chroma"], (cb, cr)):
+            pl = np.ascontiguousarray(pl)
+            assert pl.shape == (chh, cw)
+            cu.check(cu.L.x265cu_copy2d(cu.ctx, buf.ptr + corg, cs * self.es, pl.ctypes.data, cw * self.es, cw * self.es, chh, 0))
+            cu.check(cu.L.x265cu_extend_border(cu.ctx, self.depth, buf.ptr + corg, cs, cw, chh, CMARGIN_X, CMARGIN_Y))
+        f["cstride"], f["corg"] = cs, corg
+
+    def _wp_frame(self, i):
+        from .lib import WpFrame
+        f = self.fr[i]
+        if not f.get("wp_valid"):
+            raise ValueError("frame %d has no picture statistics: init_frame it with aq={...}" % i)
+        r = WpFrame()
+        for k in range(4):
+            r.lowres[k] = f["planes"][k].ptr + self.lorg
+        r.lowresStride = self.ls
+        if f.get("chroma") is not None:
+            r.cb, r.cr = f["chroma"][0].ptr + f["corg"], f["chroma"][1].ptr + f["corg"]
+            r.chromaStride = f["cstride"]
+        for k in range(3):
+            r.wp_sum[k], r.wp_ssd[k] = int(f["wp_sum"][k]), int(f["wp_ssd"][k])
+        r.poc = i
+        return r
+
+    def weight_analyse(self, b, slice_type, refs, bframes, num_ref_idx):
+        """weightAnalyse (encoder/weightPrediction.cpp:222-539) of frame b as a P (slice_type "P", refs = [ref0]) or B
+        ("B", refs = [ref0, ref1]) slice, on what the window holds: the lowres planes, intraCost, the motion fields
+        lowresMvs[list][|b - ref|] (those the estimates searched), wp_sum / wp_ssd (init_frame(aq=...)) and, in 4:2:0,
+        the chroma kept by init_frame(keep_chroma=True) (4:0:0 when frame b has none).  Window indices are the pocs.
+        num_ref_idx: Slice::m_numRefIdx per list.  Returns the [2][16][3][4] int32 table of {wtPresent, inputWeight,
+        log2WeightDenom, inputOffset}; entries the reference does not write stay 0."""
+        import ctypes as C
+        from .lib import WpParams, WpFrame
+        cu = self.cu
+        nl = 1 if slice_type == "P" else 2
+        assert len(refs) == nl and self.fr[b]["has_intra"]
+        csp = 1 if self.fr[b].get("chroma") is not None else 0
+        prm = WpParams(1 if nl == 1 else 0, (C.c_int32 * 2)(*(list(num_ref_idx) + [0] * (2 - len(num_ref_idx)))), bframes,
+                       self.W, self.H, csp)
+        fenc = self._wp_frame(b)
+        recs = [self._wp_frame(r) for r in refs]
+        rp = (C.POINTER(WpFrame) * 2)(*[C.pointer(r) for r in recs] + [C.POINTER(WpFrame)()] * (2 - nl))
+        mvs = (C.c_void_p * 2)()
+        for lst, r in enumerate(refs):
+            mv = self.fr[b]["mvs"].get((lst, abs(b - r)))
+            mvs[lst] = mv.ptr if mv is not None else None
+        out = np.zeros((2, 16, 3, 4), np.int32)
+        cu.check(cu.L.x265cu_weightp_analyse(cu.ctx, self.depth, C.byref(prm), C.byref(fenc), self.fr[b]["intraCost"].ptr, rp,
+                                             mvs, out.ctypes.data))
+        return out
 
     def set_invqscale(self, i, invq):
         """Lowres::invQscaleFactor of frame i (int32 per lowres CU, 256 = 1.0): the adaptive-quantisation weights that
@@ -323,6 +395,8 @@ class Lookahead:
                 f["invq"].free()
             if f["prop"] is not None:
                 f["prop"].free()
+            for buf in f.get("chroma") or []:
+                buf.free()
         self.tab.free()
         if self._full is not None:
             self._full.free()
