@@ -250,10 +250,13 @@ void* x265cu_analyser_ref_plane(x265cu_analyser*, int idx, int* stride); /* devi
 int x265cu_analyser_ref_updated(x265cu_analyser*, int idx);            /* re-extend borders after writing the plane in place */
 int x265cu_analyser_fetch(x265cu_analyser*, int what, void* host);    /* parity/debug access to resident results; what =
                                                                           16 + 16 * ref + yf * 4 + xf: the whole allocation of
-                                                                          reference ref's quarter-pel phase plane (xf, yf) */
+                                                                          reference ref's quarter-pel phase plane (xf, yf), of
+                                                                          its weighted plane when it is weighted
+                                                                          (x265cu_analyser_set_ref_weights) */
 /* Every reference of an analyser is stored with its 15 quarter-pel phase planes, which every ME run rebuilds for the
  * sub-pel refinement: 15 planes of (width + 192, 64-aligned) x (height + 160) pixels per reference, e.g. 561 MB at
- * 3840x2160 8-bit with 4 references, 1.40 GB at 3840x2160 10-bit with 5, 5.3 GB at 7680x4320 10-bit with 5. */
+ * 3840x2160 8-bit with 4 references, 1.40 GB at 3840x2160 10-bit with 5, 5.3 GB at 7680x4320 10-bit with 5.  A weighted
+ * reference adds a second block of 16 (x265cu_analyser_set_ref_weights). */
 /* CTU-row shards (BASELINE configs[4]: WPP CTU rows sharded per GPU; the reference enables row r once the reference
  * rows it needs are reconstructed, frameencoder.cpp:850-868, producer side framefilter.cpp:664).  All job / CU / TU
  * lists are in CTU raster order, so rows [ctuRow0, ctuRow1) are one contiguous slice of every result array
@@ -597,6 +600,31 @@ int x265cu_weightp_decide(int depth, const x265cu_wp_params* params, const x265c
 int x265cu_weightp_analyse(x265cu_ctx*, int depth, const x265cu_wp_params* params, const x265cu_wp_frame* fenc,
                            const int32_t* intraCost_dev, const x265cu_wp_frame* const* refs, const int32_t* const* mvs_dev,
                            x265cu_wp_entry* out);
+
+/* ---------- weighted P-slice references of the frame analyser ----------
+ * Applies one reference's weights, as x265cu_weightp_analyse's [0][idx] row gives them (m_weightPredTable[0][idx][0..2]:
+ * luma, Cb, Cr), to the analyses of a P slice whose list 0 is the analyser's references.  The reference is weighted iff
+ * w[0].wtPresent (frameencoder.cpp:550, predict.cpp:94); w == NULL or w[0].wtPresent == 0 makes it unweighted again, and the
+ * results are then those of an analyser that was never weighted.  For a weighted reference:
+ *   - the motion search (pre-checks, integer search, sub-pel phases) reads a weighted copy of its luma plane, and the
+ *     chroma-SATD term a weighted copy of each chroma plane whose own wtPresent is set (at subme > 2): MotionReference::init
+ *     and applyWeight (reference.cpp:51-185), weight_pp with w = inputWeight, offset = inputOffset << (depth - 8), shift =
+ *     denom + 14 - depth, round = (denom ? 1 << (denom - 1) : 0) << (14 - depth), borders replicated;
+ *   - the residual stages (bits 1 and 3) predict a CU that chose it from its unweighted planes in 14-bit precision, then
+ *     weight_sp with addWeightUni's shift = denom + 14 - depth and round = 1 << (shift - 1) (predict.cpp:82-112, 525-578);
+ *     chroma uses entries 1 and 2 whatever their wtPresent.  The choice of reference is unchanged.
+ * ref_plane / ref_plane_chroma, recon_to_ref* and ref_updated / ref_chroma_updated keep addressing the unweighted planes; the
+ * weighted copies are rebuilt from them at the start of the next run after any change.  They cover the whole picture and
+ * its margins, so row runs give the entries of a full-frame run.  x265cu_analyser_fetch code 16 + 16 * ref + phase returns
+ * what the search reads (the weighted block of a weighted reference), x265cu_analyser_fetch_chroma code 10 + 2 * numRefs +
+ * 2 * ref + plane the chroma plane the chroma-SATD term reads.
+ * Memory: a weighted reference gets its own block of 16 luma planes (the weighted plane and its 15 phases), allocated on first
+ * use and kept until destroy: 150 MB at 3840x2160 8-bit, 300 MB at 10-bit; plus one chroma plane (2.3 / 4.7 MB) per weighted
+ * chroma plane.
+ * Returns -1 before any state change (x265cu_last_error) for idx outside 0..numRefs - 1 or an entry with wtPresent not 0 / 1,
+ * log2WeightDenom outside 0..7, inputWeight outside -128..255 or inputOffset outside -128..127.  Only P slices: B-slice
+ * weights (weightb, addWeightBi) are not applied. */
+int x265cu_analyser_set_ref_weights(x265cu_analyser*, int idx, const x265cu_wp_entry w[3]);
 
 #ifdef __cplusplus
 }

@@ -55,6 +55,15 @@ struct x265cu_analyser
     int16_t* d_coefC[2]; uint8_t* d_reconC[4][2]; void** d_reconCTable;
     unsigned long long* d_cu_sseC; uint32_t* d_cu_numsigC;
     std::vector<GeoRect> rowReachC;       // per CTU row, the chroma pixels its chroma MC can read (geometry_chroma_reach)
+    // weighted P-slice references (x265cu_analyser_set_ref_weights): wp = the caller's m_weightPredTable[0][r] row, all zero
+    // for an unweighted reference.  A weighted reference gets its own ME block d_wrefs[r] (slot 0 its weighted plane, slots
+    // 1..15 that plane's phases) and, for each weighted chroma plane, d_wrefC[r][plane], allocated on first use.  wDirty[r]:
+    // the weighted planes of r no longer match its pixels or weights; the next run rebuilds them (an_weights_prepare).  While
+    // nWeighted > 0 the search reads d_meRefTable / d_meCbTable / d_meCrTable and the residual stages d_wtab ([16][3]
+    // {weighted, w0, offset, shift}); d_wjobs holds the weight_pp band jobs of every (reference, plane).
+    x265cu_wp_entry wp[16][3]; int nWeighted, wDirty[16];
+    uint8_t* d_wrefs[16]; uint8_t* d_wrefC[16][2];
+    void** d_meRefTable; void** d_meCbTable; void** d_meCrTable; int4* d_wtab; x265cu_blk_job* d_wjobs;
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -189,6 +198,111 @@ static bool an_chroma_reach_ok(const x265cu_analyser* a, int r0, int r1)
     return geometry_chroma_reach_inside(u, a->p.width, a->p.height, a->cstride, AN_MARGIN_X / 2, AN_MARGIN_Y / 2);
 }
 
+// ---- weighted references: MotionReference::init / applyWeight (encoder/reference.cpp:51-185) on the resident planes ----
+static bool an_ref_weighted(const x265cu_analyser* a, int r) { return a->wp[r][0].wtPresent != 0; }
+// chroma plane c (1 Cb, 2 Cr) of reference r is weighted for the search when the reference is (frameencoder.cpp:550), the
+// plane's own wtPresent is set and the search has the chroma-SATD term (numInterpPlanes = 3 at subme > 2, reference.cpp:57)
+static bool an_refc_weighted(const x265cu_analyser* a, int r, int c)
+{
+    return an_ref_weighted(a, r) && a->chromaOn && a->p.subme > 2 && a->wp[r][c].wtPresent;
+}
+
+static int an_band_jobs(int h) { return (h + 15) / 16; }
+
+// applyWeight's result once every row is weighted: weight_pp of the picture (w = inputWeight, round = (denom ? 1 << (denom - 1)
+// : 0) << (14 - depth), shift = denom + 14 - depth, offset = inputOffset << (depth - 8)), then the borders replicated as its
+// extendRowBorder and the above / below copies do.  One weight_pp job per 16-row band, in jobs (device, an_band_jobs(h)).
+static int an_weight_plane(x265cu_analyser* a, const uint8_t* src, uint8_t* dst, int stride, int w, int h, int mx, int my,
+                           const x265cu_wp_entry& e, x265cu_blk_job* jobs)
+{
+    const int depth = a->p.depth, corr = 14 - depth, denom = e.log2WeightDenom;
+    std::vector<x265cu_blk_job> hj(an_band_jobs(h));
+    for (size_t j = 0; j < hj.size(); j++)
+    {
+        x265cu_blk_job& b = hj[j];
+        memset(&b, 0, sizeof(b));
+        b.d_off = b.a_off = (int64_t)j * 16 * stride;
+        b.d_stride = b.a_stride = b.b_stride = stride;
+        b.w = (int16_t)w; b.h = (int16_t)min(16, h - (int)j * 16);
+        b.p0 = e.inputWeight; b.p1 = (denom ? 1 << (denom - 1) : 0) << corr; b.p2 = denom + corr; b.p3 = e.inputOffset * (1 << (depth - 8));
+    }
+    CU_CHECK(cudaMemcpy(jobs, hj.data(), sizeof(x265cu_blk_job) * hj.size(), cudaMemcpyHostToDevice));
+    if (launch_blockop(a->ctx, depth, X265CU_WEIGHT_PP, dst, src, NULL, jobs, (int)hj.size())) return -1;
+    return x265cu_extend_border(a->ctx, depth, dst, stride, w, h, mx, my);
+}
+
+static uint8_t* an_alloc_zeroed(x265cu_ctx* c, size_t bytes)
+{
+    uint8_t* d = (uint8_t*)x265cu_malloc(c, bytes);
+    if (d && cudaMemset(d, 0, bytes) != cudaSuccess) return NULL;
+    return d;
+}
+
+// Brings the weighted planes, the search's pointer tables, the tensor maps and the residual weight table up to date with the
+// references changed since the last run (wDirty).  Nothing runs while no reference has ever been weighted.
+static int an_weights_prepare(x265cu_analyser* a)
+{
+    x265cu_ctx* c = a->ctx;
+    const int n = a->p.numRefs, depth = a->p.depth;
+    const size_t es = depth == 8 ? 1 : 2;
+    bool dirty = false;
+    for (int r = 0; r < n; r++) dirty = dirty || a->wDirty[r];
+    if (!dirty) return 0;
+    CU_CHECK(cudaStreamSynchronize(c->stream));          // no launch still reads the job lists and tables rewritten below
+    const int lj = an_band_jobs(a->p.height), cj = an_band_jobs(a->p.height >> 1);
+    if (!a->d_wjobs) a->d_wjobs = (x265cu_blk_job*)x265cu_malloc(c, sizeof(x265cu_blk_job) * (size_t)16 * (lj + 2 * cj));
+    if (!a->d_meRefTable) a->d_meRefTable = (void**)x265cu_malloc(c, sizeof(void*) * 16);
+    if (!a->d_meCbTable) a->d_meCbTable = (void**)x265cu_malloc(c, sizeof(void*) * 16);
+    if (!a->d_meCrTable) a->d_meCrTable = (void**)x265cu_malloc(c, sizeof(void*) * 16);
+    if (!a->d_wtab) a->d_wtab = (int4*)x265cu_malloc(c, sizeof(int4) * 48);
+    if (!a->d_wjobs || !a->d_meRefTable || !a->d_meCbTable || !a->d_meCrTable || !a->d_wtab) return -1;
+    void* me[16] = {}; void* mc[2][16] = {}; int4 wt[48] = {};
+    for (int r = 0; r < n; r++)
+    {
+        const bool wl = an_ref_weighted(a, r);
+        x265cu_blk_job* jobs = a->d_wjobs + (size_t)r * (lj + 2 * cj);
+        if (wl && !a->d_wrefs[r] && !(a->d_wrefs[r] = an_alloc_zeroed(c, 16 * a->planeBytes)))
+        {
+            x265cu_set_error("analyser: no device memory for a weighted reference and its 15 phase planes", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+            return -1;
+        }
+        if (wl && a->wDirty[r] && an_weight_plane(a, a->d_refs[r] + a->orgBytes, a->d_wrefs[r] + a->orgBytes, a->stride, a->p.width,
+                                                  a->p.height, AN_MARGIN_X, AN_MARGIN_Y, a->wp[r][0], jobs)) return -1;
+        me[r] = (wl ? a->d_wrefs[r] : a->d_refs[r]) + a->orgBytes;
+        for (int k = 0; k < 2 && a->chromaOn; k++)
+        {
+            const bool wc = an_refc_weighted(a, r, k + 1);
+            if (wc && !a->d_wrefC[r][k] && !(a->d_wrefC[r][k] = an_alloc_zeroed(c, a->cPlaneBytes)))
+            {
+                x265cu_set_error("analyser: no device memory for a weighted chroma reference plane", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+                return -1;
+            }
+            if (wc && a->wDirty[r] && an_weight_plane(a, a->d_refC[r][k] + a->cOrgBytes, a->d_wrefC[r][k] + a->cOrgBytes, a->cstride,
+                                                      a->p.width >> 1, a->p.height >> 1, AN_MARGIN_X / 2, AN_MARGIN_Y / 2, a->wp[r][k + 1],
+                                                      jobs + lj + k * cj)) return -1;
+            mc[k][r] = (wc ? a->d_wrefC[r][k] : a->d_refC[r][k]) + a->cOrgBytes;
+        }
+        if (a->windowOn && a->wDirty[r])
+        {
+            CUtensorMap tm[MEW_NCLS];
+            if (mew_build_tmaps(wl ? a->d_wrefs[r] : a->d_refs[r], a->stride, a->planeRows, (int)es, tm)) return -1;
+            CU_CHECK(cudaMemcpy(a->d_tmaps + (size_t)r * MEW_NCLS, tm, sizeof(tm), cudaMemcpyHostToDevice));
+        }
+        for (int p = 0; p < 3; p++)
+            wt[3 * r + p] = make_int4(wl, a->wp[r][p].inputWeight, a->wp[r][p].inputOffset * (1 << (depth - 8)),
+                                      a->wp[r][p].log2WeightDenom + 14 - depth);
+        a->wDirty[r] = 0;
+    }
+    CU_CHECK(cudaMemcpy(a->d_meRefTable, me, sizeof(void*) * 16, cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemcpy(a->d_meCbTable, mc[0], sizeof(void*) * 16, cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemcpy(a->d_meCrTable, mc[1], sizeof(void*) * 16, cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemcpy(a->d_wtab, wt, sizeof(wt), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// the pixels of reference idx changed: its weighted planes are rebuilt before the next run
+static void an_ref_changed(x265cu_analyser* a, int idx) { if (an_ref_weighted(a, idx)) a->wDirty[idx] = 1; }
+
 // the residual stage of the luma plane or of both 4:2:0 chroma planes over the CUs [cu0, cu0 + ncu) and their TUs, the
 // CTU rows [r0, r1)
 static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int r0, int r1)
@@ -211,7 +325,8 @@ static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int r0
     CU_CHECK(cudaMemsetAsync(r.cu_numsig + (size_t)npl * cu0, 0, sizeof(uint32_t) * npl * ncu, c->stream));
     const int32_t* lists[3]; int n[3];
     for (int k = 0; k < 3; k++) { lists[k] = a->d_tuBy[k] + a->rowTuBy[k][r0]; n[k] = a->rowTuBy[k][r1] - a->rowTuBy[k][r0]; }
-    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r, lists, n) : launch_resid<uint16_t>(c, chroma, r, lists, n);
+    const int4* wt = a->nWeighted ? a->d_wtab : nullptr;
+    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r, lists, n, wt) : launch_resid<uint16_t>(c, chroma, r, lists, n, wt);
 }
 
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
@@ -240,6 +355,7 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
     const int ntu = a->rowTu[r1] - a->rowTu[r0];
+    if (an_weights_prepare(a)) return -1;
     a->ev_valid = stages;
     CU_CHECK(cudaEventRecord(a->ev[0], c->stream));
     if ((stages & 1) && nj > 0)
@@ -251,7 +367,8 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         if (a->chromaOn)
         {
             ch.fencCb = a->d_fencC[0] + a->cOrgBytes; ch.fencCr = a->d_fencC[1] + a->cOrgBytes;
-            ch.refCb = (const void* const*)a->d_refCbTable; ch.refCr = (const void* const*)a->d_refCrTable; ch.cstride = a->cstride;
+            ch.refCb = (const void* const*)(a->nWeighted ? a->d_meCbTable : a->d_refCbTable);
+            ch.refCr = (const void* const*)(a->nWeighted ? a->d_meCrTable : a->d_refCrTable); ch.cstride = a->cstride;
         }
         MeWinLaunch win;
         if (a->windowOn)
@@ -270,9 +387,9 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         }
         MePlanes pl;
         pl.nrefs = a->p.numRefs; pl.ppitch = (ptrdiff_t)(a->planeBytes / (depth == 8 ? 1 : 2));
-        for (int r = 0; r < a->p.numRefs; r++) pl.blocks[r] = a->d_refs[r];
+        for (int r = 0; r < a->p.numRefs; r++) pl.blocks[r] = an_ref_weighted(a, r) ? a->d_wrefs[r] : a->d_refs[r];
         for (int g = 0; g < 3; g++) { pl.jobs[g] = a->d_planeJobs[g]; pl.njobs[g] = a->nPlaneJobs[g]; }
-        if (launch_me(c, depth, a->d_fenc + a->orgBytes, a->stride, (const void* const*)a->d_refTable, a->stride, 0,
+        if (launch_me(c, depth, a->d_fenc + a->orgBytes, a->stride, (const void* const*)(a->nWeighted ? a->d_meRefTable : a->d_refTable), a->stride, 0,
                       a->d_mvcost + a->mvrange, a->d_jobs + job0, nj, a->d_me_out + (size_t)job0 * 4, c->d_counter,
                       a->chromaOn ? &ch : NULL, a->windowOn ? &win : NULL, &pl)) return -1;
         CU_CHECK(cudaEventRecord(a->ev[4], c->stream));      // ME search kernel alone ends here
@@ -433,6 +550,8 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     cudaFree(a->d_refCbTable); cudaFree(a->d_refCrTable);
     for (int k = 0; k < 2; k++) { cudaFree(a->d_coefC[k]); for (int d = 0; d < 4; d++) cudaFree(a->d_reconC[d][k]); }
     cudaFree(a->d_reconCTable); cudaFree(a->d_cu_sseC); cudaFree(a->d_cu_numsigC);
+    for (int r = 0; r < 16; r++) { cudaFree(a->d_wrefs[r]); cudaFree(a->d_wrefC[r][0]); cudaFree(a->d_wrefC[r][1]); }
+    cudaFree(a->d_meRefTable); cudaFree(a->d_meCbTable); cudaFree(a->d_meCrTable); cudaFree(a->d_wtab); cudaFree(a->d_wjobs);
     x265cu_host_free(a->h_fenc); x265cu_host_free(a->h_field);
     delete a;
 }
@@ -446,6 +565,7 @@ int x265cu_analyser_counts(x265cu_analyser* a, int* njobs, int* ncu, int* ntu, i
 int x265cu_analyser_set_ref(x265cu_analyser* a, int idx, const void* host_luma, int host_stride)
 {
     if (idx < 0 || idx >= a->p.numRefs) return -1;
+    an_ref_changed(a, idx);
     if (an_upload_plane(a, a->d_refs[idx], host_luma, host_stride)) return -1;
     return x265cu_sync(a->ctx);
 }
@@ -507,12 +627,14 @@ int x265cu_analyser_enable_chroma(x265cu_analyser* a)
     CU_CHECK(cudaMemcpy(a->d_refCbTable, cbt, sizeof(void*) * a->p.numRefs, cudaMemcpyHostToDevice));
     CU_CHECK(cudaMemcpy(a->d_refCrTable, crt, sizeof(void*) * a->p.numRefs, cudaMemcpyHostToDevice));
     a->chromaOn = 1;
+    for (int r = 0; r < a->p.numRefs; r++) an_ref_changed(a, r);
     return 0;
 }
 
 int x265cu_analyser_set_ref_chroma(x265cu_analyser* a, int idx, const void* cb_host, const void* cr_host, int host_stride)
 {
     if (!a->chromaOn || idx < 0 || idx >= a->p.numRefs) return -1;
+    an_ref_changed(a, idx);
     if (an_upload_cplane(a, a->d_refC[idx][0], cb_host, host_stride) || an_upload_cplane(a, a->d_refC[idx][1], cr_host, host_stride)) return -1;
     return x265cu_sync(a->ctx);
 }
@@ -592,16 +714,25 @@ int x265cu_analyser_chroma_results(x265cu_analyser* a, int ctuRow0, int ctuRow1,
 }
 
 // what: 0 / 1 the Cb / Cr levels (ncoef / 4 each); 2 + 2 * depthIdx + plane the whole allocation of a chroma recon plane,
-// 10 + 2 * ref + plane the whole allocation of a reference's chroma plane (cstride x (height / 2 + 80) elements each)
+// 10 + 2 * ref + plane the whole allocation of a reference's chroma plane (cstride x (height / 2 + 80) elements each);
+// 10 + 2 * numRefs + 2 * ref + plane the chroma plane the chroma-SATD term of the search reads for the reference: its weighted
+// plane when it has one, else the reference's plane (needs enable_chroma only)
 int x265cu_analyser_fetch_chroma(x265cu_analyser* a, int what, void* host)
 {
-    if (!a->chromaResOn || what < 0 || what >= 10 + 2 * a->p.numRefs) return -1;
+    const int nr = a->p.numRefs;
+    if (!a->chromaOn || what < 0 || what >= 10 + 4 * nr || (what < 10 + 2 * nr && !a->chromaResOn)) return -1;
     x265cu_ctx* c = a->ctx;
     const size_t es = a->p.depth == 8 ? 1 : 2, planeBytes = (size_t)a->cstride * a->cRows * es;
     const void* src; size_t bytes;
     if (what < 2) { src = a->d_coefC[what]; bytes = sizeof(int16_t) * (a->ncoef / 4); }
     else if (what < 10) { src = a->d_reconC[(what - 2) >> 1][what & 1]; bytes = planeBytes; }
-    else { src = a->d_refC[(what - 10) >> 1][what & 1]; bytes = planeBytes; }
+    else if (what < 10 + 2 * nr) { src = a->d_refC[(what - 10) >> 1][what & 1]; bytes = planeBytes; }
+    else
+    {
+        const int r = (what - 10 - 2 * nr) >> 1, k = what & 1;
+        if (an_weights_prepare(a)) return -1;
+        src = an_refc_weighted(a, r, k + 1) ? a->d_wrefC[r][k] : a->d_refC[r][k]; bytes = planeBytes;
+    }
     cudaSetDevice(c->device);
     CU_CHECK(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));
@@ -625,6 +756,7 @@ int x265cu_analyser_recon_to_ref_chroma(x265cu_analyser* a, int depthIdx, int id
     const int ch = a->p.height >> 1, y0 = ctuRow0 * 32, y1 = ctuRow1 * 32 < ch ? ctuRow1 * 32 : ch;
     cudaSetDevice(a->ctx->device);
     const size_t off = a->cOrgBytes + (size_t)y0 * a->cstride * es, pitch = (size_t)a->cstride * es;
+    an_ref_changed(a, idx);
     for (int k = 0; k < 2; k++)
         CU_CHECK(cudaMemcpy2DAsync(a->d_refC[idx][k] + off, pitch, a->d_reconC[depthIdx][k] + off, pitch, (size_t)(a->p.width >> 1) * es, y1 - y0,
                                    cudaMemcpyDeviceToDevice, a->ctx->stream));
@@ -636,6 +768,7 @@ int x265cu_analyser_ref_chroma_updated(x265cu_analyser* a, int idx)
 {
     if (!a->chromaOn || idx < 0 || idx >= a->p.numRefs) return -1;
     cudaSetDevice(a->ctx->device);
+    an_ref_changed(a, idx);
     for (int k = 0; k < 2; k++)
         if (x265cu_extend_border(a->ctx, a->p.depth, a->d_refC[idx][k] + a->cOrgBytes, a->cstride, a->p.width >> 1, a->p.height >> 1,
                                  AN_MARGIN_X / 2, AN_MARGIN_Y / 2)) return -1;
@@ -726,6 +859,7 @@ int x265cu_analyser_ref_updated(x265cu_analyser* a, int idx)
 {
     if (idx < 0 || idx >= a->p.numRefs) return -1;
     cudaSetDevice(a->ctx->device);
+    an_ref_changed(a, idx);
     return x265cu_extend_border(a->ctx, a->p.depth, a->d_refs[idx] + a->orgBytes, a->stride, a->p.width, a->p.height, AN_MARGIN_X, AN_MARGIN_Y);
 }
 
@@ -746,6 +880,7 @@ int x265cu_analyser_recon_to_ref(x265cu_analyser* a, int depthIdx, int idx, int 
     const int y0 = ctuRow0 * 64, y1 = ctuRow1 * 64 < a->p.height ? ctuRow1 * 64 : a->p.height;
     cudaSetDevice(a->ctx->device);
     const size_t off = a->orgBytes + (size_t)y0 * a->stride * es, pitch = (size_t)a->stride * es;
+    an_ref_changed(a, idx);
     CU_CHECK(cudaMemcpy2DAsync(a->d_refs[idx] + off, pitch, a->d_recon[depthIdx] + off, pitch, (size_t)a->p.width * es, y1 - y0,
                                cudaMemcpyDeviceToDevice, a->ctx->stream));
     return 0;
@@ -767,12 +902,40 @@ int x265cu_analyser_fetch(x265cu_analyser* a, int what, void* host)
     case 7: src = a->d_cu_jobs; bytes = sizeof(int32_t) * a->ncu * a->p.numRefs; break;
     case 8: src = a->d_fenc; bytes = (size_t)a->stride * a->planeRows * es; break;
     default:
-        // 16 + 16 * ref + phase: the whole allocation of phase plane yf * 4 + xf of reference `ref` (phase 0 = the reference)
+        // 16 + 16 * ref + phase: the whole allocation of phase plane yf * 4 + xf of what the search reads for reference `ref`
+        // (phase 0 = the plane itself): its weighted block when it is weighted, else the reference's
         if (what < 16 || what >= 16 + 16 * a->p.numRefs) return -1;
-        src = a->d_refs[(what - 16) >> 4] + (size_t)((what - 16) & 15) * a->planeBytes; bytes = (size_t)a->stride * a->planeRows * es;
+        {
+            const int r = (what - 16) >> 4;
+            if (an_weights_prepare(a)) return -1;
+            src = (an_ref_weighted(a, r) ? a->d_wrefs[r] : a->d_refs[r]) + (size_t)((what - 16) & 15) * a->planeBytes;
+            bytes = (size_t)a->stride * a->planeRows * es;
+        }
     }
     CU_CHECK(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// Weighted prediction of reference idx (list 0 of a P slice): w = m_weightPredTable[0][idx][0..2] (luma, Cb, Cr), NULL or
+// w[0].wtPresent == 0 = unweighted.  Refused before any state change: a bad index or entry (x265cu_last_error).
+int x265cu_analyser_set_ref_weights(x265cu_analyser* a, int idx, const x265cu_wp_entry* w)
+{
+    const char* bad = NULL;
+    if (idx < 0 || idx >= a->p.numRefs) bad = "x265cu_analyser_set_ref_weights: reference index outside 0..numRefs - 1";
+    for (int k = 0; k < 3 && w && !bad; k++)
+    {
+        if (w[k].wtPresent != 0 && w[k].wtPresent != 1) bad = "x265cu_analyser_set_ref_weights: wtPresent not 0 or 1";
+        else if (w[k].log2WeightDenom < 0 || w[k].log2WeightDenom > 7) bad = "x265cu_analyser_set_ref_weights: log2WeightDenom outside 0..7";
+        else if (w[k].inputWeight < -128 || w[k].inputWeight > 255) bad = "x265cu_analyser_set_ref_weights: inputWeight outside -128..255";
+        else if (w[k].inputOffset < -128 || w[k].inputOffset > 127) bad = "x265cu_analyser_set_ref_weights: inputOffset outside -128..127";
+    }
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
+    const bool on = w && w[0].wtPresent, was = an_ref_weighted(a, idx);
+    if (!on && !was) return 0;
+    for (int k = 0; k < 3; k++) a->wp[idx][k] = on ? w[k] : x265cu_wp_entry{};
+    a->nWeighted += (int)on - (int)was;
+    a->wDirty[idx] = 1;
     return 0;
 }
 

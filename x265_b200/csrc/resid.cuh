@@ -68,8 +68,14 @@ struct ResidArgs
 
 // Item j of [0, NPL * ntu) = plane j % NPL of TU tul[j / NPL].  NT = 8 is the luma plane, NT = 4 the two chroma planes at half
 // resolution.  Every TU of the list is at most MAXS wide in the launch's planes.
-template <typename P, int TPJ, int MAXS, int NT>
-__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const ResidArgs a)
+// WT: the P-slice weighted uni-prediction (Predict::motionCompensation with wp0->wtPresent, predict.cpp:82-112).  wt[3 * ref +
+// plane] = {weighted, w0, offset, shift}: weighted = the reference's luma wtPresent (the same in its three entries), w0 =
+// inputWeight, offset = inputOffset << (depth - 8), shift = log2WeightDenom + 14 - depth.  A CU whose reference is weighted
+// takes the 14-bit prediction of the unweighted plane (predInterLumaShort / predInterChromaShort) and weight_sp with
+// addWeightUni's round 1 << (shift - 1) (predict.cpp:525-578, pixel.cpp:493-516); chroma uses entries 1 and 2 whatever
+// their wtPresent.  WT = false compiles to the unweighted stage alone.
+template <typename P, int TPJ, int MAXS, int NT, bool WT>
+__device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __restrict__ wt)
 {
     constexpr int DEPTH = PixTraits<P>::depth, maxv = PixTraits<P>::maxv;
     constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ, NPL = NT == 8 ? 1 : 2, SUB = NPL - 1;
@@ -109,7 +115,19 @@ __global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const Res
         const P* fe = (const P*)(plane ? a.fenc[1] : a.fenc[0]) + off;
         pc_sync<TPJ>();                                           // the previous item's tiles have been read
         for (int i = t; i < N; i += TPJ) M[i] = d_dct[lg - 2][i];
-        pc_predict<P, TPJ, MAXS, NT, false>(ref, a.stride, mo[1], mo[2], T, T, s_pred, s_win, s_mid, t);
+        if (WT && wt[3 * best].x)
+        {
+            pc_predict<P, TPJ, MAXS, NT, true>(ref, a.stride, mo[1], mo[2], T, T, s_pred, s_win, s_mid, t);
+            pc_sync<TPJ>();
+            const int4 w = wt[3 * best + SUB + plane];             // luma entry 0, Cb / Cr entries 1 / 2
+            for (int i = t; i < N; i += TPJ)
+            {
+                const int y = i >> lg, x = i & (T - 1);
+                s_pred[y * DP + x] = (int16_t)clip3i(0, maxv, ((w.y * ((int)s_pred[y * DP + x] + 8192) + (1 << (w.w - 1))) >> w.w) + w.z);
+            }
+        }
+        else
+            pc_predict<P, TPJ, MAXS, NT, false>(ref, a.stride, mo[1], mo[2], T, T, s_pred, s_win, s_mid, t);
         pc_sync<TPJ>();
         // ---- residual ----
         for (int i = t; i < N; i += TPJ)
@@ -209,28 +227,43 @@ __global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const Res
 }
 
 template <typename P, int TPJ, int MAXS, int NT>
-static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a)
+__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual(const ResidArgs a)
+{
+    cu_residual<P, TPJ, MAXS, NT, false>(a, nullptr);
+}
+
+// the stage of a frame with at least one weighted reference (the unweighted ones take the same path as in k_cu_residual)
+template <typename P, int TPJ, int MAXS, int NT>
+__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual_wp(const ResidArgs a, const int4* __restrict__ wt)
+{
+    cu_residual<P, TPJ, MAXS, NT, true>(a, wt);
+}
+
+template <typename P, int TPJ, int MAXS, int NT>
+static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a, const int4* wt)
 {
     constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ;
     const int items = (NT == 8 ? 1 : 2) * a.ntu;
     if (items == 0) return 0;
-    k_cu_residual<P, TPJ, MAXS, NT><<<min((items + JPB - 1) / JPB, c->sm_count * maxPerSm), TPJ > 128 ? TPJ : 128, 0, c->stream>>>(a);
+    const int grid = min((items + JPB - 1) / JPB, c->sm_count * maxPerSm), block = TPJ > 128 ? TPJ : 128;
+    if (wt) k_cu_residual_wp<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a, wt);
+    else    k_cu_residual<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a);
     CU_LAUNCH_CHECK(c);
     return 0;
 }
 
 // One launch per luma TU size, each over its own list (lists[k] = TUs of luma size 8 << k, n[k] entries): luma TUs of 8 a
 // warp each, of 16 a 128-thread CTA, of 32 a 256-thread CTA (at most 8 per SM); chroma TUs of 4 and 8 a warp each, of 16 a
-// 128-thread CTA; at most 16 CTAs per SM otherwise
+// 128-thread CTA; at most 16 CTAs per SM otherwise.  wt (device, [16][3]) non-null: the weighted stage (k_cu_residual_wp).
 template <typename P>
-static int launch_resid(x265cu_ctx* c, bool chroma, ResidArgs a, const int32_t* const lists[3], const int n[3])
+static int launch_resid(x265cu_ctx* c, bool chroma, ResidArgs a, const int32_t* const lists[3], const int n[3], const int4* wt = nullptr)
 {
     for (int k = 0; k < 3; k++)
     {
         a.tul = lists[k]; a.ntu = n[k];
-        const int e = chroma ? (k < 2 ? resid_launch<P, 32, 8, 4>(c, 16, a) : resid_launch<P, 128, 16, 4>(c, 16, a))
-                             : (k == 0 ? resid_launch<P, 32, 8, 8>(c, 16, a) : k == 1 ? resid_launch<P, 128, 16, 8>(c, 16, a)
-                                                                                     : resid_launch<P, 256, 32, 8>(c, 8, a));
+        const int e = chroma ? (k < 2 ? resid_launch<P, 32, 8, 4>(c, 16, a, wt) : resid_launch<P, 128, 16, 4>(c, 16, a, wt))
+                             : (k == 0 ? resid_launch<P, 32, 8, 8>(c, 16, a, wt) : k == 1 ? resid_launch<P, 128, 16, 8>(c, 16, a, wt)
+                                                                                         : resid_launch<P, 256, 32, 8>(c, 8, a, wt));
         if (e) return -1;
     }
     return 0;

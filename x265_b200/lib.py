@@ -381,6 +381,7 @@ _AN_PROTOS = {
     "x265cu_analyser_ref_chroma_updated": (I, [P, I]),
     "x265cu_analyser_ref_plane_chroma": (P, [P, I, I, C.POINTER(I)]),
     "x265cu_analyser_src_plane": (P, [P, I, C.POINTER(I)]),
+    "x265cu_analyser_set_ref_weights": (I, [P, I, P]),
 }
 STAGE_CHROMA_RESIDUAL = 8                 # analyser stage bit 3 (x265cu_analyser_enable_chroma_residual)
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
@@ -595,6 +596,25 @@ class Analyser:
         st = I()
         return self.lib.L.x265cu_analyser_recon_plane_chroma(self.h, depth_idx, plane, C.byref(st)), st.value
 
+    # ---- weighted P-slice references (x265cu_analyser_set_ref_weights) ----
+    def set_ref_weights(self, idx, entries):
+        """Weights of reference idx: a (3, 4) int array {wtPresent, inputWeight, log2WeightDenom, inputOffset} for luma, Cb, Cr
+        as Lookahead.weight_analyse()[0][idx] returns it, or None (unweighted)."""
+        if entries is None:
+            self.lib.check(self.lib.L.x265cu_analyser_set_ref_weights(self.h, idx, None))
+            return
+        e = np.ascontiguousarray(entries, np.int32)
+        assert e.shape == (3, 4), e.shape
+        self.lib.check(self.lib.L.x265cu_analyser_set_ref_weights(self.h, idx, e.ctypes.data))
+
+    def fetch_search_chroma(self, ref, plane):
+        """The whole allocation of the chroma plane (0 Cb, 1 Cr) that the chroma-SATD term of the search reads for reference
+        ref: its weighted plane when it has one, else the reference's plane."""
+        assert 0 <= ref < self.numRefs and plane in (0, 1)
+        out = np.zeros(self.chroma_plane_shape(), self.dtype)
+        self.lib.check(self.lib.L.x265cu_analyser_fetch_chroma(self.h, 10 + 2 * self.numRefs + 2 * ref + plane, out.ctypes.data))
+        return out
+
     def recon_to_ref_chroma(self, depth_idx, ref_idx, r0, r1):
         self.lib.check(self.lib.L.x265cu_analyser_recon_to_ref_chroma(self.h, depth_idx, ref_idx, r0, r1))
 
@@ -637,7 +657,8 @@ class Analyser:
 
     def fetch(self, what):
         """A device-resident array by name, or ("plane", ref, phase): the whole allocation (stride x (height + 160)) of
-        reference ref's phase plane yf * 4 + xf (phase 0 = the reference plane itself)."""
+        reference ref's phase plane yf * 4 + xf (phase 0 = the reference plane itself; for a weighted reference, of its weighted
+        plane: what the search reads)."""
         es = np.dtype(self.dtype).itemsize
         rows = self.height + 160
         if isinstance(what, tuple):
