@@ -219,7 +219,7 @@ int x265cu_pred_cost_batch(x265cu_ctx*, int depth, const void* fenc_dev, int fen
  * reference, the motionEstimate() result (motion.cpp:739), for every CU the residual-coding stats of
  * its best 2Nx2N prediction (search.cpp:3178; quant.cpp:397-470, 543-605) and its 35 intra SA8D costs
  * (search.cpp:1358-1444).  stages: bit0 ME, bit1 residual, bit2 intra, bit3 chroma residual (see
- * x265cu_analyser_enable_chroma_residual). */
+ * x265cu_analyser_enable_chroma_residual), bit4 BIDIR of a B slice (see x265cu_analyser_set_lists). */
 typedef struct x265cu_analyser x265cu_analyser;
 typedef struct {
     int width, height, depth, numRefs;
@@ -623,8 +623,49 @@ int x265cu_weightp_analyse(x265cu_ctx*, int depth, const x265cu_wp_params* param
  * chroma plane.
  * Returns -1 before any state change (x265cu_last_error) for idx outside 0..numRefs - 1 or an entry with wtPresent not 0 / 1,
  * log2WeightDenom outside 0..7, inputWeight outside -128..255 or inputOffset outside -128..127.  Only P slices: B-slice
- * weights (weightb, addWeightBi) are not applied. */
+ * weights (weightb, addWeightBi) are not applied, and a run of a B slice (x265cu_analyser_set_lists) is refused while any
+ * reference is weighted. */
 int x265cu_analyser_set_ref_weights(x265cu_analyser*, int idx, const x265cu_wp_entry w[3]);
+
+/* ---------- B slices of the frame analyser ----------
+ * x265cu_analyser_set_lists splits the analyser's numRefs reference slots into the slice's two lists: slots [0, numRefL0)
+ * are list-0 refIdx 0..numRefL0 - 1, slots [numRefL0, numRefs) list-1 refIdx 0..numRefL1 - 1.  A picture in both lists (GPB,
+ * low-delay B) is loaded into two slots, each with its own predictor plane, as the encoder searches it twice.  numRefL1 == 0
+ * is a P slice: the state at creation, whose results are those of an analyser that never saw a B slice.  The ME stage and
+ * its job list do not change: every slot is searched.  Returns -1 before any state change (x265cu_last_error) unless
+ * numRefL0 >= 1, numRefL1 >= 0 and numRefL0 + numRefL1 == numRefs.
+ *
+ * Stage bit 4 (value 16), BIDIR: Analysis::checkInter_rd0_4 for 2Nx2N and checkBidir2Nx2N (analysis.cpp:3062-3071,
+ * 3145-3265) for every CU (8 to 64), on the analyser's own cost model:
+ *   1. per list, the CU's 2Nx2N job of lowest ME cost over that list's slots (ties to the lowest slot); the uni-directional
+ *      winner is list 0 if cost0 <= cost1, else list 1 (search.cpp:2611);
+ *   2. uniCost = sa8d of the winner's pixel prediction (predInterLumaPixel), + sa8d(Cb) + sa8d(Cr) of its chroma prediction
+ *      when chroma is enabled (x265cu_analyser_enable_chroma; the chroma SA8D of a CU 8 is satd 4x4, primitives.cpp:185-188),
+ *      + mvcost(mv - mvp) of the winner;
+ *   3. biCost = sa8d of addAvg(predInterLumaShort(L0 best), predInterLumaShort(L1 best)) (+ the chroma twin) + mvcost0(mv0 -
+ *      mvp0) + mvcost1(mv1 - mvp1), each MVP the MVP of that job;
+ *   4. the zero pair is tried if either vector is nonzero and both MVPs lie in setSearchRange(cu, 0, max(width, height)) (the
+ *      clip of the ME job build, then mvmax.y += 2 and both bounds << 2); zCost, the same formula with both vectors zero,
+ *      replaces biCost and the pair if zCost < biCost;
+ *   5. the CU is bi-predicted iff biCost < uniCost.
+ * The bits model is the analyser's: the only bits term is the ME's mvcost table (x265cu_mvcost_table at the analyser's lambda,
+ * the sum of the two components truncated to 16 bits as the ME's).  No reference-index, list-selection or MVP-index bits and
+ * no checkBestMVP: those belong to the host's AMVP and CABAC state.
+ * On a B slice the residual stages (bits 1 and 3) code the decision: a CU with interDir 1 or 2 takes its winning slot as on
+ * a P slice; a CU with interDir 3 predicts every TU through the two 14-bit predictions and addAvg (predict.cpp:168-189), then
+ * runs the unchanged chain, and its cu_ref is its list-0 slot.
+ * Refused with -1 before any launch: value 16 on a P slice; value 2 or 8 on a B slice without value 16 in the same call; any
+ * run of a B slice while a reference is weighted (x265cu_analyser_set_ref_weights). */
+typedef struct {
+    uint32_t uniCost, biCost;   /* step 2, and step 3 after the zero try */
+    int8_t   interDir;          /* 1 L0, 2 L1, 3 bi */
+    int8_t   ref[2];            /* slot of the best L0 / L1 2Nx2N job */
+    uint8_t  zero;              /* 1: the zero pair replaced the searched pair */
+    int16_t  mv[2][2];          /* the bi pair's quarter-pel vectors */
+} x265cu_bidir_cu;
+int x265cu_analyser_set_lists(x265cu_analyser*, int numRefL0, int numRefL1);
+/* the BIDIR records of the CTU rows [ctuRow0, ctuRow1) into `out`, a full-frame host array of ncu records (synchronous) */
+int x265cu_analyser_bidir_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x265cu_bidir_cu* out);
 
 #ifdef __cplusplus
 }

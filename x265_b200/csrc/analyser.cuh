@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include "frame.cuh"
 #include "resid.cuh"
+#include "bidir.cuh"
 #include "me.cuh"
 #include "me_window.cuh"
 #include <vector>
@@ -26,7 +27,7 @@ struct x265cu_analyser
     int16_t* d_coef; unsigned long long* d_cu_sse; uint32_t* d_cu_numsig; int32_t* d_cu_ref; uint32_t* d_intra;
     // pinned host staging for the e2e path
     uint8_t* h_fenc; int16_t* h_field;
-    cudaEvent_t ev[5]; int ev_valid;      // stage boundaries of the last an_run (ME build+search+pack | residual | intra)
+    cudaEvent_t ev[6]; int ev_valid;      // stage boundaries of the last an_run (ME build+search+pack | BIDIR | residual | intra)
     std::vector<PuDesc> pus; std::vector<CuDesc> cus; std::vector<TuDesc> tus; std::vector<int32_t> cu_jobs;
     // first PU job / CU / TU of every CTU row (+ one past the end): the lists are in CTU raster order, so a CTU-row
     // range [r0, r1) is one contiguous slice of each list (what a WPP row shard owns, frameencoder.cpp:850-868)
@@ -64,6 +65,9 @@ struct x265cu_analyser
     x265cu_wp_entry wp[16][3]; int nWeighted, wDirty[16];
     uint8_t* d_wrefs[16]; uint8_t* d_wrefC[16][2];
     void** d_meRefTable; void** d_meCbTable; void** d_meCrTable; int4* d_wtab; x265cu_blk_job* d_wjobs;
+    // B slices (x265cu_analyser_set_lists): slots [0, numRefL0) are list 0, the rest list 1 (numRefL1 == 0: a P slice);
+    // d_bidir = the BIDIR stage's record of every CU (stage bit 4), allocated by the first set_lists with a list 1
+    int numRefL0, numRefL1; x265cu_bidir_cu* d_bidir;
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -198,6 +202,15 @@ static bool an_chroma_reach_ok(const x265cu_analyser* a, int r0, int r1)
     return geometry_chroma_reach_inside(u, a->p.width, a->p.height, a->cstride, AN_MARGIN_X / 2, AN_MARGIN_Y / 2);
 }
 
+// the chroma reach of every CTU row (built once, on the first stage that needs it)
+static void an_build_chroma_reach(x265cu_analyser* a)
+{
+    if (!a->rowReachC.empty()) return;
+    a->rowReachC.resize(a->ctuRows);
+    for (int r = 0; r < a->ctuRows; r++)
+        a->rowReachC[r] = geometry_chroma_reach(a->p.width, a->p.height, a->cus, a->tus, a->rowTu[r], a->rowTu[r + 1]);
+}
+
 // ---- weighted references: MotionReference::init / applyWeight (encoder/reference.cpp:51-185) on the resident planes ----
 static bool an_ref_weighted(const x265cu_analyser* a, int r) { return a->wp[r][0].wtPresent != 0; }
 // chroma plane c (1 Cb, 2 Cr) of reference r is weighted for the search when the reference is (frameencoder.cpp:550), the
@@ -326,7 +339,8 @@ static int an_residual(x265cu_analyser* a, bool chroma, int cu0, int ncu, int r0
     const int32_t* lists[3]; int n[3];
     for (int k = 0; k < 3; k++) { lists[k] = a->d_tuBy[k] + a->rowTuBy[k][r0]; n[k] = a->rowTuBy[k][r1] - a->rowTuBy[k][r0]; }
     const int4* wt = a->nWeighted ? a->d_wtab : nullptr;
-    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r, lists, n, wt) : launch_resid<uint16_t>(c, chroma, r, lists, n, wt);
+    const x265cu_bidir_cu* bd = a->numRefL1 ? a->d_bidir : nullptr;   // a B slice: the BIDIR records of this same run
+    return a->p.depth == 8 ? launch_resid<uint8_t>(c, chroma, r, lists, n, wt, bd) : launch_resid<uint16_t>(c, chroma, r, lists, n, wt, bd);
 }
 
 // Runs the stages over the CTU rows [r0, r1).  Every list is sliced by pointer offset only: PU jobs, ME results and
@@ -352,6 +366,20 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         x265cu_set_error("analyser: the phase planes do not cover the rows the sub-pel search can read", cudaErrorInvalidValue, __FILE__, __LINE__);
         return -1;
     }
+    const char* bad = NULL;
+    if ((stages & 16) && !a->numRefL1) bad = "analyser: stage bit 4 (BIDIR) needs a B slice (x265cu_analyser_set_lists with numRefL1 > 0)";
+    else if (a->numRefL1 && (stages & 10) && !(stages & 16))
+        bad = "analyser: the residual stages of a B slice (bits 1, 3) need stage bit 4 (BIDIR) in the same call";
+    else if (a->numRefL1 && a->nWeighted) bad = "analyser: B-slice weights are not applied; clear every reference's weights first";
+    // Reach of the BIDIR stage and of the bi residual: every vector they use is an ME result of a CU's 2Nx2N job, which
+    // k_build_me_jobs' clip bounds as it bounds the vectors of the uni residual, or zero.  Their luma reads are the 8-tap
+    // windows of those vectors on the reference planes, inside what an_planes_cover checks for the sub-pel search (which
+    // reads the same vectors' windows); their chroma reads are the 4-tap windows of the CU's chroma block, the union of its
+    // TUs' blocks, inside what an_chroma_reach_ok checks for the chroma residual.
+    else if ((stages & 16) && !an_planes_cover(a, r0, r1)) bad = "analyser: the reference planes do not cover what the BIDIR stage can read";
+    else if ((stages & 16) && a->chromaOn && (an_build_chroma_reach(a), !an_chroma_reach_ok(a, r0, r1)))
+        bad = "analyser: the chroma planes do not cover what the BIDIR stage's chroma MC can read";
+    if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
     const int ntu = a->rowTu[r1] - a->rowTu[r0];
@@ -398,6 +426,22 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     }
     else if (stages & 1) CU_CHECK(cudaEventRecord(a->ev[4], c->stream));
     CU_CHECK(cudaEventRecord(a->ev[1], c->stream));
+    if ((stages & 16) && ncu > 0)
+    {
+        BidirArgs b;
+        b.fenc[0] = a->d_fenc + a->orgBytes; b.refs[0] = a->d_refTable; b.stride = a->stride; b.chroma = a->chromaOn;
+        for (int k = 0; k < 2 && a->chromaOn; k++)
+        {
+            b.fenc[1 + k] = a->d_fencC[k] + a->cOrgBytes; b.refs[1 + k] = k ? a->d_refCrTable : a->d_refCbTable;
+        }
+        b.cstride = a->cstride;
+        b.cus = a->d_cus; b.cu_jobs = a->d_cu_jobs; b.numRefs = a->p.numRefs; b.numRefL0 = a->numRefL0; b.me_out = a->d_me_out;
+        b.jobs = a->d_jobs; b.mvc = a->d_mvcost + a->mvrange; b.width = a->p.width; b.height = a->p.height; b.out = a->d_bidir;
+        const int32_t* lists[4]; int n[4];
+        for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
+        if (depth == 8 ? launch_bidir<uint8_t>(c, b, lists, n) : launch_bidir<uint16_t>(c, b, lists, n)) return -1;
+    }
+    CU_CHECK(cudaEventRecord(a->ev[5], c->stream));
     if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, r0, r1)) return -1;
     CU_CHECK(cudaEventRecord(a->ev[2], c->stream));
     if ((stages & 4) && ncu > 0)
@@ -483,6 +527,7 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     a->d_mvcost = an_upload(ctx, tab);
     a->d_pus = an_upload(ctx, a->pus); a->d_cus = an_upload(ctx, a->cus); a->d_tus = an_upload(ctx, a->tus); a->d_cu_jobs = an_upload(ctx, a->cu_jobs);
     a->d_jobs = (x265cu_me_job*)x265cu_malloc(ctx, sizeof(x265cu_me_job) * a->njobs);
+    if (a->d_jobs) cudaMemset(a->d_jobs, 0, sizeof(x265cu_me_job) * a->njobs);     // the MVPs a BIDIR run before any search reads
     a->d_me_out = (int32_t*)x265cu_malloc(ctx, sizeof(int32_t) * 4 * a->njobs);
     // a residual stage run before any search reads vector 0 of every CU, which lies inside every plane's reach
     if (a->d_me_out) cudaMemset(a->d_me_out, 0, sizeof(int32_t) * 4 * a->njobs);
@@ -513,7 +558,8 @@ x265cu_analyser* x265cu_analyser_create(x265cu_ctx* ctx, const x265cu_analysis_p
     a->d_cu_numsig = (uint32_t*)x265cu_malloc(ctx, sizeof(uint32_t) * a->ncu);
     a->d_cu_ref = (int32_t*)x265cu_malloc(ctx, sizeof(int32_t) * a->ncu);
     a->d_intra = (uint32_t*)x265cu_malloc(ctx, sizeof(uint32_t) * 36 * a->ncu);
-    for (int i = 0; i < 5; i++) cudaEventCreate(&a->ev[i]);
+    for (int i = 0; i < 6; i++) cudaEventCreate(&a->ev[i]);
+    a->numRefL0 = p->numRefs; a->numRefL1 = 0;
     a->ev_valid = 0;
     a->chromaOn = 0; a->d_refCbTable = a->d_refCrTable = NULL;
     a->d_fencC[0] = a->d_fencC[1] = NULL;
@@ -552,6 +598,7 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     cudaFree(a->d_reconCTable); cudaFree(a->d_cu_sseC); cudaFree(a->d_cu_numsigC);
     for (int r = 0; r < 16; r++) { cudaFree(a->d_wrefs[r]); cudaFree(a->d_wrefC[r][0]); cudaFree(a->d_wrefC[r][1]); }
     cudaFree(a->d_meRefTable); cudaFree(a->d_meCbTable); cudaFree(a->d_meCrTable); cudaFree(a->d_wtab); cudaFree(a->d_wjobs);
+    cudaFree(a->d_bidir);
     x265cu_host_free(a->h_fenc); x265cu_host_free(a->h_field);
     delete a;
 }
@@ -660,9 +707,7 @@ int x265cu_analyser_enable_chroma_residual(x265cu_analyser* a, int cbQpOffset, i
     a->qpC[0] = geometry_chroma_qp(a->p.qp, cbQpOffset, a->p.depth);
     a->qpC[1] = geometry_chroma_qp(a->p.qp, crQpOffset, a->p.depth);
     if (a->chromaResOn) return 0;
-    a->rowReachC.resize(a->ctuRows);
-    for (int r = 0; r < a->ctuRows; r++)
-        a->rowReachC[r] = geometry_chroma_reach(a->p.width, a->p.height, a->cus, a->tus, a->rowTu[r], a->rowTu[r + 1]);
+    an_build_chroma_reach(a);
     if (!an_chroma_reach_ok(a, 0, a->ctuRows))
     {
         x265cu_set_error("x265cu_analyser_enable_chroma_residual: the chroma planes do not cover what the chroma MC can read", cudaErrorInvalidValue, __FILE__, __LINE__);
@@ -840,7 +885,7 @@ int x265cu_analyser_analyse(x265cu_analyser* a, const void* fenc_host, int host_
 int x265cu_analyser_stage_ms(x265cu_analyser* a, float* ms)
 {
     CU_CHECK(cudaEventSynchronize(a->ev[3]));
-    for (int i = 0; i < 3; i++) CU_CHECK(cudaEventElapsedTime(&ms[i], a->ev[i], a->ev[i + 1]));
+    for (int i = 0; i < 3; i++) CU_CHECK(cudaEventElapsedTime(&ms[i], a->ev[i == 1 ? 5 : i], a->ev[i + 1]));   // [1] from after BIDIR
     ms[3] = 0.f;
     if (a->ev_valid & 1) CU_CHECK(cudaEventElapsedTime(&ms[3], a->ev[0], a->ev[4]));
     return 0;
@@ -936,6 +981,45 @@ int x265cu_analyser_set_ref_weights(x265cu_analyser* a, int idx, const x265cu_wp
     for (int k = 0; k < 3; k++) a->wp[idx][k] = on ? w[k] : x265cu_wp_entry{};
     a->nWeighted += (int)on - (int)was;
     a->wDirty[idx] = 1;
+    return 0;
+}
+
+// Lists of a B slice: slots [0, numRefL0) list 0, [numRefL0, numRefs) list 1; numRefL1 == 0 a P slice.  Refused before
+// any state change unless numRefL0 >= 1, numRefL1 >= 0 and numRefL0 + numRefL1 == numRefs.
+int x265cu_analyser_set_lists(x265cu_analyser* a, int numRefL0, int numRefL1)
+{
+    if (numRefL0 < 1 || numRefL1 < 0 || numRefL0 + numRefL1 != a->p.numRefs)
+    {
+        x265cu_set_error("x265cu_analyser_set_lists: needs numRefL0 >= 1, numRefL1 >= 0 and numRefL0 + numRefL1 == numRefs", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    if (numRefL1 && !a->d_bidir)
+    {
+        cudaSetDevice(a->ctx->device);
+        a->d_bidir = (x265cu_bidir_cu*)an_alloc_zeroed(a->ctx, sizeof(x265cu_bidir_cu) * a->ncu);
+        if (!a->d_bidir)
+        {
+            x265cu_set_error("x265cu_analyser_set_lists: no device memory for the BIDIR records", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+            return -1;
+        }
+    }
+    a->numRefL0 = numRefL0; a->numRefL1 = numRefL1;
+    return 0;
+}
+
+// the BIDIR records of the CTU rows [r0, r1) into a full-frame sized host array (synchronous)
+int x265cu_analyser_bidir_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, x265cu_bidir_cu* out)
+{
+    if (!a->d_bidir || ctuRow0 < 0 || ctuRow1 > a->ctuRows || ctuRow0 > ctuRow1)
+    {
+        x265cu_set_error("x265cu_analyser_bidir_results: no B slice set, or a bad CTU row range", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    x265cu_ctx* c = a->ctx;
+    cudaSetDevice(c->device);
+    const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
+    if (nc) CU_CHECK(cudaMemcpyAsync(out + c0, a->d_bidir + c0, sizeof(x265cu_bidir_cu) * nc, cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
     return 0;
 }
 

@@ -74,8 +74,12 @@ struct ResidArgs
 // takes the 14-bit prediction of the unweighted plane (predInterLumaShort / predInterChromaShort) and weight_sp with
 // addWeightUni's round 1 << (shift - 1) (predict.cpp:525-578, pixel.cpp:493-516); chroma uses entries 1 and 2 whatever
 // their wtPresent.  WT = false compiles to the unweighted stage alone.
-template <typename P, int TPJ, int MAXS, int NT, bool WT>
-__device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __restrict__ wt)
+// BI: a B slice (the BIDIR stage's record bd[cu], bidir.cuh).  A CU with interDir 3 predicts each TU through the two 14-bit
+// predictions of its list-0 / list-1 slots at its pair of vectors and addAvg (predict.cpp:168-189, pixel.cpp:842-862); its
+// cu_ref is its list-0 slot.  Any other CU takes the path above: its uni-directional winner is the lowest ME cost over all
+// slots, ties to the lowest, because the list-0 slots come first.
+template <typename P, int TPJ, int MAXS, int NT, bool WT, bool BI = false>
+__device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __restrict__ wt, const x265cu_bidir_cu* __restrict__ bd = nullptr)
 {
     constexpr int DEPTH = PixTraits<P>::depth, maxv = PixTraits<P>::maxv;
     constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ, NPL = NT == 8 ? 1 : 2, SUB = NPL - 1;
@@ -84,7 +88,7 @@ __device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __re
     // to MAXS + 2 so that the column reads of the forward passes fall in distinct banks.
     constexpr int TP = MAXS + 2, MC = WR * (MAXS + 8) + WR * MAXS, TILES = 2 * MAXS * TP;
     constexpr int SCR = MC > TILES ? MC : TILES, DP = MAXS;
-    __shared__ int16_t s_all[JPB][SCR + MAXS * MAXS];
+    __shared__ int16_t s_all[JPB][SCR + (BI ? 2 : 1) * MAXS * MAXS];   // BI: the list-1 prediction after s_pred
     __shared__ int8_t s_mat[JPB][MAXS * MAXS];                    // the TU size's DCT matrix
     __shared__ int s_red[TPJ / 32];
     __shared__ unsigned long long s_red64[TPJ / 32];
@@ -109,13 +113,33 @@ __device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __re
             const int cost = a.me_out[(size_t)a.cu_jobs[tu.cu * a.numRefs + r] * 4];
             if (cost < bcost) { bcost = cost; best = r; }
         }
+        const bool bi = BI && bd[tu.cu].interDir == 3;
+        if (bi) best = bd[tu.cu].ref[0];
         const int32_t* mo = a.me_out + (size_t)a.cu_jobs[tu.cu * a.numRefs + best] * 4;
         const ptrdiff_t off = (ptrdiff_t)pt.y * a.stride + pt.x;
         const P* ref = ((const P* const*)(plane ? a.refs[1] : a.refs[0]))[best] + off;
         const P* fe = (const P*)(plane ? a.fenc[1] : a.fenc[0]) + off;
         pc_sync<TPJ>();                                           // the previous item's tiles have been read
         for (int i = t; i < N; i += TPJ) M[i] = d_dct[lg - 2][i];
-        if (WT && wt[3 * best].x)
+        if (bi)
+        {
+            // the record's words 2..4: {interDir, ref[0], ref[1], zero}, mv[0] (x | y << 16), mv[1]
+            const int* w = reinterpret_cast<const int*>(bd + tu.cu);
+            const int rw = w[2], v0 = w[3], v1 = w[4];
+            const P* const* tab = (const P* const*)(plane ? a.refs[1] : a.refs[0]);
+            int16_t* s_p1 = s_pred + MAXS * MAXS;
+            pc_predict<P, TPJ, MAXS, NT, true>(tab[(int8_t)(rw >> 8)] + off, a.stride, (v0 << 16) >> 16, v0 >> 16, T, T, s_pred, s_win, s_mid, t);
+            pc_sync<TPJ>();
+            pc_predict<P, TPJ, MAXS, NT, true>(tab[(int8_t)(rw >> 16)] + off, a.stride, (v1 << 16) >> 16, v1 >> 16, T, T, s_p1, s_win, s_mid, t);
+            pc_sync<TPJ>();
+            constexpr int shift = 15 - DEPTH, offset = (1 << (shift - 1)) + 2 * 8192;
+            for (int i = t; i < N; i += TPJ)
+            {
+                const int y = i >> lg, x = i & (T - 1);
+                s_pred[y * DP + x] = (int16_t)clip3i(0, maxv, ((int)s_pred[y * DP + x] + (int)s_p1[y * DP + x] + offset) >> shift);
+            }
+        }
+        else if (WT && wt[3 * best].x)
         {
             pc_predict<P, TPJ, MAXS, NT, true>(ref, a.stride, mo[1], mo[2], T, T, s_pred, s_win, s_mid, t);
             pc_sync<TPJ>();
@@ -239,14 +263,22 @@ __global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual_wp(const 
     cu_residual<P, TPJ, MAXS, NT, true>(a, wt);
 }
 
+// the stage of a B slice (bd = the BIDIR records; the uni-predicted CUs take the same path as in k_cu_residual)
 template <typename P, int TPJ, int MAXS, int NT>
-static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a, const int4* wt)
+__global__ void __launch_bounds__(TPJ > 128 ? TPJ : 128) k_cu_residual_bi(const ResidArgs a, const x265cu_bidir_cu* __restrict__ bd)
+{
+    cu_residual<P, TPJ, MAXS, NT, false, true>(a, nullptr, bd);
+}
+
+template <typename P, int TPJ, int MAXS, int NT>
+static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a, const int4* wt, const x265cu_bidir_cu* bd)
 {
     constexpr int JPB = (TPJ > 128 ? TPJ : 128) / TPJ;
     const int items = (NT == 8 ? 1 : 2) * a.ntu;
     if (items == 0) return 0;
     const int grid = min((items + JPB - 1) / JPB, c->sm_count * maxPerSm), block = TPJ > 128 ? TPJ : 128;
-    if (wt) k_cu_residual_wp<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a, wt);
+    if (bd) k_cu_residual_bi<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a, bd);
+    else if (wt) k_cu_residual_wp<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a, wt);
     else    k_cu_residual<P, TPJ, MAXS, NT><<<grid, block, 0, c->stream>>>(a);
     CU_LAUNCH_CHECK(c);
     return 0;
@@ -254,16 +286,18 @@ static int resid_launch(x265cu_ctx* c, int maxPerSm, const ResidArgs& a, const i
 
 // One launch per luma TU size, each over its own list (lists[k] = TUs of luma size 8 << k, n[k] entries): luma TUs of 8 a
 // warp each, of 16 a 128-thread CTA, of 32 a 256-thread CTA (at most 8 per SM); chroma TUs of 4 and 8 a warp each, of 16 a
-// 128-thread CTA; at most 16 CTAs per SM otherwise.  wt (device, [16][3]) non-null: the weighted stage (k_cu_residual_wp).
+// 128-thread CTA; at most 16 CTAs per SM otherwise.  wt (device, [16][3]) non-null: the weighted stage (k_cu_residual_wp);
+// bd (device, [ncu]) non-null: the stage of a B slice (k_cu_residual_bi).
 template <typename P>
-static int launch_resid(x265cu_ctx* c, bool chroma, ResidArgs a, const int32_t* const lists[3], const int n[3], const int4* wt = nullptr)
+static int launch_resid(x265cu_ctx* c, bool chroma, ResidArgs a, const int32_t* const lists[3], const int n[3], const int4* wt = nullptr,
+                        const x265cu_bidir_cu* bd = nullptr)
 {
     for (int k = 0; k < 3; k++)
     {
         a.tul = lists[k]; a.ntu = n[k];
-        const int e = chroma ? (k < 2 ? resid_launch<P, 32, 8, 4>(c, 16, a, wt) : resid_launch<P, 128, 16, 4>(c, 16, a, wt))
-                             : (k == 0 ? resid_launch<P, 32, 8, 8>(c, 16, a, wt) : k == 1 ? resid_launch<P, 128, 16, 8>(c, 16, a, wt)
-                                                                                         : resid_launch<P, 256, 32, 8>(c, 8, a, wt));
+        const int e = chroma ? (k < 2 ? resid_launch<P, 32, 8, 4>(c, 16, a, wt, bd) : resid_launch<P, 128, 16, 4>(c, 16, a, wt, bd))
+                             : (k == 0 ? resid_launch<P, 32, 8, 8>(c, 16, a, wt, bd) : k == 1 ? resid_launch<P, 128, 16, 8>(c, 16, a, wt, bd)
+                                                                                             : resid_launch<P, 256, 32, 8>(c, 8, a, wt, bd));
         if (e) return -1;
     }
     return 0;

@@ -384,6 +384,12 @@ _AN_PROTOS = {
     "x265cu_analyser_set_ref_weights": (I, [P, I, P]),
 }
 STAGE_CHROMA_RESIDUAL = 8                 # analyser stage bit 3 (x265cu_analyser_enable_chroma_residual)
+STAGE_BIDIR = 16                          # analyser stage bit 4: BIDIR of a B slice (x265cu_analyser_set_lists)
+_AN_PROTOS["x265cu_analyser_set_lists"] = (I, [P, I, I])
+_AN_PROTOS["x265cu_analyser_bidir_results"] = (I, [P, I, I, P])
+# x265cu_bidir_cu (include/x265_b200.h)
+BIDIR_CU = np.dtype([("uniCost", np.uint32), ("biCost", np.uint32), ("interDir", np.int8), ("ref", np.int8, 2), ("zero", np.uint8),
+                     ("mv", np.int16, (2, 2))])
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
 _AN_PROTOS["x265cu_lowres_intra_batch"] = (I, [P, I, P, I, I, I, I, I])
 _AN_PROTOS["x265cu_lookahead_cost_batch"] = (I, [P, I, P, I, I, I, I, P])
@@ -573,6 +579,21 @@ class Analyser:
         assert sse.shape == numsig.shape == (self.ncu, 2) and sse.dtype == np.uint64 and numsig.dtype == np.uint32
         self.lib.check(self.lib.L.x265cu_analyser_chroma_results(self.h, r0, r1, sse.ctypes.data, numsig.ctypes.data))
         return sse, numsig
+
+    # ---- B slices (x265cu_analyser_set_lists, stage bit 4) ----
+    def set_lists(self, n0, n1):
+        """Slots [0, n0) are list 0, [n0, n0 + n1) list 1 (n0 + n1 == numRefs); n1 == 0 is a P slice.  Afterwards runs may
+        set stage bit 4 (STAGE_BIDIR), and a B slice's residual stages need it in the same call."""
+        self.lib.check(self.lib.L.x265cu_analyser_set_lists(self.h, n0, n1))
+
+    def bidir_results(self, r0=0, r1=None, out=None):
+        """The BIDIR record (BIDIR_CU) of every CU of the CTU rows [r0, r1) (default: all) into the given full-frame array or
+        a new zeroed one; returns it."""
+        r1 = self.ctu_rows if r1 is None else r1
+        out = np.zeros(self.ncu, BIDIR_CU) if out is None else out
+        assert out.shape == (self.ncu,) and out.dtype == BIDIR_CU
+        self.lib.check(self.lib.L.x265cu_analyser_bidir_results(self.h, r0, r1, out.ctypes.data))
+        return out
 
     def chroma_plane_shape(self):
         """(rows, cstride) of a chroma plane allocation: the picture's origin is at row 40, column 48."""
