@@ -219,7 +219,8 @@ int x265cu_pred_cost_batch(x265cu_ctx*, int depth, const void* fenc_dev, int fen
  * reference, the motionEstimate() result (motion.cpp:739), for every CU the residual-coding stats of
  * its best 2Nx2N prediction (search.cpp:3178; quant.cpp:397-470, 543-605) and its 35 intra SA8D costs
  * (search.cpp:1358-1444).  stages: bit0 ME, bit1 residual, bit2 intra, bit3 chroma residual (see
- * x265cu_analyser_enable_chroma_residual), bit4 BIDIR of a B slice (see x265cu_analyser_set_lists). */
+ * x265cu_analyser_enable_chroma_residual), bit4 BIDIR of a B slice (see x265cu_analyser_set_lists), bit5 PART of a P slice
+ * (see x265cu_analyser_part_results). */
 typedef struct x265cu_analyser x265cu_analyser;
 typedef struct {
     int width, height, depth, numRefs;
@@ -666,6 +667,37 @@ typedef struct {
 int x265cu_analyser_set_lists(x265cu_analyser*, int numRefL0, int numRefL1);
 /* the BIDIR records of the CTU rows [ctuRow0, ctuRow1) into `out`, a full-frame host array of ncu records (synchronous) */
 int x265cu_analyser_bidir_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x265cu_bidir_cu* out);
+
+/* ---------- inter estimate of every partition of a P slice's CUs ----------
+ * Stage bit 5 (value 32), PART: the sa8dCost of checkInter_rd0_4 (analysis.cpp:3023-3071) for every partition the analyser's
+ * geometry emits for every CU (8 to 64): 2Nx2N always, 2NxN and Nx2N with rect, 2NxnU, 2NxnD, nLx2N and nRx2N with amp at
+ * CU >= 16 -- what compressInterCU_rd0_4 compares (analysis.cpp:1439-1593).  On the analyser's cost model:
+ *   1. each PU takes the slot of lowest ME cost among its jobs, ties to the lowest slot (PU k of CU c for slot r is job
+ *      cu_jobs[c * numRefs + r] + k, k in the geometry's order: 2Nx2N; 2NxN x2; Nx2N x2; 2NxnU x2; 2NxnD x2; nLx2N x2;
+ *      nRx2N x2), so the 2Nx2N entry's slot is the residual stage's cu_ref;
+ *   2. each PU is predicted at its ME vector into the CU's S x S prediction: predInterLumaPixel, and with chroma enabled
+ *      (x265cu_analyser_enable_chroma) predInterChromaPixel of its (pw/2) x (ph/2) chroma block (the vector read as eighth-pel);
+ *      a weighted slot (x265cu_analyser_set_ref_weights) takes predInterLumaShort / predInterChromaShort of its unweighted
+ *      planes and addWeightUni, as the residual stages do (predict.cpp:82-112);
+ *   3. sa8d = cu[S].sa8d of the luma prediction, + chroma[I420].cu[S].sa8d of Cb and of Cr when chroma is enabled (satd 4x4
+ *      for a CU 8); cost = sa8d + the sum over the partition's PUs of mvcost(mv - mvp), the MVP the job's, each PU's two
+ *      components summed to 16 bits as in the ME.
+ * As in BIDIR there are no reference-index, MVP-index or list bits, no checkBestMVP and no merge estimation of the rect /
+ * AMP PUs, and nothing is gated by split cost or thresholds: every emitted partition is evaluated and the host decides.
+ * One record per CU, read with x265cu_analyser_part_results; the records are allocated zeroed by the first value-32 run.
+ * Refused with -1 before any launch: value 32 on a B slice (numRefL1 > 0: a B slice's rect / AMP PUs need predInterSearch's
+ * per-PU list choice and bi-prediction).  Every vector used is the ME result of one of the CU's PU jobs, which
+ * k_build_me_jobs' clip bounds relative to the CU origin, and every PU lies inside its CU, so the reads stay inside what
+ * an_planes_cover (luma) and an_chroma_reach_ok (chroma) check; a value-32 run where either fails is refused too. */
+typedef struct {
+    uint32_t cost[8];      /* indexed by PartSize (SIZE_2Nx2N 0 .. SIZE_nRx2N 7); UINT32_MAX where not evaluated (NxN always) */
+    uint32_t sa8d[8];      /* the distortion part of cost; UINT32_MAX where not evaluated */
+    int8_t   ref[8][2];    /* slot of PU 0 / PU 1; -1 where there is no such PU */
+    int16_t  mv[8][2][2];  /* quarter-pel vector of each PU; 0 where there is no such PU */
+} x265cu_part_cu;          /* 144 bytes */
+/* the PART records of the CTU rows [ctuRow0, ctuRow1) into `out`, a full-frame host array of ncu records (synchronous);
+ * refused before any value-32 run and for a bad row range */
+int x265cu_analyser_part_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x265cu_part_cu* out);
 
 #ifdef __cplusplus
 }

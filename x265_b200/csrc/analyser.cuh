@@ -5,6 +5,7 @@
 #include "frame.cuh"
 #include "resid.cuh"
 #include "bidir.cuh"
+#include "part.cuh"
 #include "me.cuh"
 #include "me_window.cuh"
 #include <vector>
@@ -68,6 +69,8 @@ struct x265cu_analyser
     // B slices (x265cu_analyser_set_lists): slots [0, numRefL0) are list 0, the rest list 1 (numRefL1 == 0: a P slice);
     // d_bidir = the BIDIR stage's record of every CU (stage bit 4), allocated by the first set_lists with a list 1
     int numRefL0, numRefL1; x265cu_bidir_cu* d_bidir;
+    // the PART stage's record of every CU (stage bit 5), allocated zeroed by the first run with that bit
+    x265cu_part_cu* d_part;
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -379,11 +382,26 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     else if ((stages & 16) && !an_planes_cover(a, r0, r1)) bad = "analyser: the reference planes do not cover what the BIDIR stage can read";
     else if ((stages & 16) && a->chromaOn && (an_build_chroma_reach(a), !an_chroma_reach_ok(a, r0, r1)))
         bad = "analyser: the chroma planes do not cover what the BIDIR stage's chroma MC can read";
+    // Reach of the PART stage: every vector it uses is the ME result of one of the CU's PU jobs, which k_build_me_jobs' clip
+    // bounds relative to the CU origin, the same for every PU of the CU; each PU lies inside its CU.  Its luma reads are the
+    // 8-tap windows of the PUs' blocks at those vectors, the windows the sub-pel search reads for the same jobs, inside what
+    // an_planes_cover checks per PU; its chroma reads are the 4-tap windows of the PUs' chroma blocks, inside the CU's chroma
+    // block (the union of its TUs' blocks) moved by a vector inside the same clip, which an_chroma_reach_ok checks.
+    else if ((stages & 32) && a->numRefL1)
+        bad = "analyser: stage bit 5 (PART) needs a P slice: a B slice's rect / AMP PUs need the per-PU list choice and bi-prediction";
+    else if ((stages & 32) && !an_planes_cover(a, r0, r1)) bad = "analyser: the reference planes do not cover what the PART stage can read";
+    else if ((stages & 32) && a->chromaOn && (an_build_chroma_reach(a), !an_chroma_reach_ok(a, r0, r1)))
+        bad = "analyser: the chroma planes do not cover what the PART stage's chroma MC can read";
     if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
     const int ntu = a->rowTu[r1] - a->rowTu[r0];
     if (an_weights_prepare(a)) return -1;
+    if ((stages & 32) && !a->d_part && !(a->d_part = (x265cu_part_cu*)an_alloc_zeroed(c, sizeof(x265cu_part_cu) * a->ncu)))
+    {
+        x265cu_set_error("analyser: no device memory for the PART records", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+        return -1;
+    }
     a->ev_valid = stages;
     CU_CHECK(cudaEventRecord(a->ev[0], c->stream));
     if ((stages & 1) && nj > 0)
@@ -440,6 +458,22 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         const int32_t* lists[4]; int n[4];
         for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
         if (depth == 8 ? launch_bidir<uint8_t>(c, b, lists, n) : launch_bidir<uint16_t>(c, b, lists, n)) return -1;
+    }
+    if ((stages & 32) && ncu > 0)
+    {
+        PartArgs q;
+        q.fenc[0] = a->d_fenc + a->orgBytes; q.refs[0] = a->d_refTable; q.stride = a->stride; q.chroma = a->chromaOn;
+        for (int k = 0; k < 2 && a->chromaOn; k++)
+        {
+            q.fenc[1 + k] = a->d_fencC[k] + a->cOrgBytes; q.refs[1 + k] = k ? a->d_refCrTable : a->d_refCbTable;
+        }
+        q.cstride = a->cstride;
+        q.cus = a->d_cus; q.pus = a->d_pus; q.cu_jobs = a->d_cu_jobs; q.numRefs = a->p.numRefs; q.rect = a->p.rect; q.amp = a->p.amp;
+        q.me_out = a->d_me_out; q.jobs = a->d_jobs; q.mvc = a->d_mvcost + a->mvrange; q.wt = a->nWeighted ? a->d_wtab : nullptr;
+        q.out = a->d_part;
+        const int32_t* lists[4]; int n[4];
+        for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
+        if (depth == 8 ? launch_part<uint8_t>(c, q, lists, n) : launch_part<uint16_t>(c, q, lists, n)) return -1;
     }
     CU_CHECK(cudaEventRecord(a->ev[5], c->stream));
     if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, r0, r1)) return -1;
@@ -598,7 +632,7 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     cudaFree(a->d_reconCTable); cudaFree(a->d_cu_sseC); cudaFree(a->d_cu_numsigC);
     for (int r = 0; r < 16; r++) { cudaFree(a->d_wrefs[r]); cudaFree(a->d_wrefC[r][0]); cudaFree(a->d_wrefC[r][1]); }
     cudaFree(a->d_meRefTable); cudaFree(a->d_meCbTable); cudaFree(a->d_meCrTable); cudaFree(a->d_wtab); cudaFree(a->d_wjobs);
-    cudaFree(a->d_bidir);
+    cudaFree(a->d_bidir); cudaFree(a->d_part);
     x265cu_host_free(a->h_fenc); x265cu_host_free(a->h_field);
     delete a;
 }
@@ -1019,6 +1053,22 @@ int x265cu_analyser_bidir_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, 
     cudaSetDevice(c->device);
     const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
     if (nc) CU_CHECK(cudaMemcpyAsync(out + c0, a->d_bidir + c0, sizeof(x265cu_bidir_cu) * nc, cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// the PART records of the CTU rows [r0, r1) into a full-frame sized host array (synchronous)
+int x265cu_analyser_part_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, x265cu_part_cu* out)
+{
+    if (!a->d_part || ctuRow0 < 0 || ctuRow1 > a->ctuRows || ctuRow0 > ctuRow1)
+    {
+        x265cu_set_error("x265cu_analyser_part_results: no run with stage bit 5 (PART) yet, or a bad CTU row range", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    x265cu_ctx* c = a->ctx;
+    cudaSetDevice(c->device);
+    const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
+    if (nc) CU_CHECK(cudaMemcpyAsync(out + c0, a->d_part + c0, sizeof(x265cu_part_cu) * nc, cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));
     return 0;
 }

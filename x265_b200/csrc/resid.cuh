@@ -37,6 +37,14 @@ __device__ __forceinline__ int resid_dc_only(int dequantDc)
     return (((dequantDc + 1) >> 1) * 8 + (1 << (shift - 1))) >> shift;
 }
 
+// weight_sp of one 14-bit prediction sample with addWeightUni's round 1 << (shift - 1) (predict.cpp:525-578, pixel.cpp:493-516);
+// w = {weighted, w0, offset, shift} as in the residual stage's weight table (cu_residual below)
+template <int MAXV>
+__device__ __forceinline__ int resid_weight_sp(int v, const int4& w)
+{
+    return clip3i(0, MAXV, ((w.y * (v + 8192) + (1 << (w.w - 1))) >> w.w) + w.z);
+}
+
 // sum over the TPJ threads of a job group, in every thread of the group.  TPJ is a multiple of 32; a group of more than one
 // warp is the whole CTA.
 template <int TPJ, typename T>
@@ -147,7 +155,7 @@ __device__ __forceinline__ void cu_residual(const ResidArgs& a, const int4* __re
             for (int i = t; i < N; i += TPJ)
             {
                 const int y = i >> lg, x = i & (T - 1);
-                s_pred[y * DP + x] = (int16_t)clip3i(0, maxv, ((w.y * ((int)s_pred[y * DP + x] + 8192) + (1 << (w.w - 1))) >> w.w) + w.z);
+                s_pred[y * DP + x] = (int16_t)resid_weight_sp<maxv>((int)s_pred[y * DP + x], w);
             }
         }
         else

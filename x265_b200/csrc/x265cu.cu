@@ -410,6 +410,7 @@ static_assert(sizeof(x265cu_wp_frame) == 112 && sizeof(x265cu_wp_params) == 28 &
               sizeof(x265cu_wp_entry) == 16, "weightp records (include/x265_b200.h)");
 static_assert(sizeof(x265cu_deblock_unit) == 16 && sizeof(x265cu_deblock_params) == 24, "deblocking records (include/x265_b200.h)");
 static_assert(sizeof(x265cu_bidir_cu) == 20, "BIDIR record (include/x265_b200.h)");
+static_assert(sizeof(x265cu_part_cu) == 144, "PART record (include/x265_b200.h)");
 
 // the argument rules of the deblocking calls on one set of planes; NULL when they hold
 static const char* deblock_check(const char* fn, int depth, int width, int height, const void* luma, const void* cb,
