@@ -220,7 +220,7 @@ int x265cu_pred_cost_batch(x265cu_ctx*, int depth, const void* fenc_dev, int fen
  * its best 2Nx2N prediction (search.cpp:3178; quant.cpp:397-470, 543-605) and its 35 intra SA8D costs
  * (search.cpp:1358-1444).  stages: bit0 ME, bit1 residual, bit2 intra, bit3 chroma residual (see
  * x265cu_analyser_enable_chroma_residual), bit4 BIDIR of a B slice (see x265cu_analyser_set_lists), bit5 PART of a P slice
- * (see x265cu_analyser_part_results). */
+ * (see x265cu_analyser_part_results), bit6 PART_B of a B slice (see x265cu_analyser_part_b_results). */
 typedef struct x265cu_analyser x265cu_analyser;
 typedef struct {
     int width, height, depth, numRefs;
@@ -686,7 +686,7 @@ int x265cu_analyser_bidir_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x2
  * AMP PUs, and nothing is gated by split cost or thresholds: every emitted partition is evaluated and the host decides.
  * One record per CU, read with x265cu_analyser_part_results; the records are allocated zeroed by the first value-32 run.
  * Refused with -1 before any launch: value 32 on a B slice (numRefL1 > 0: a B slice's rect / AMP PUs need predInterSearch's
- * per-PU list choice and bi-prediction).  Every vector used is the ME result of one of the CU's PU jobs, which
+ * per-PU list choice and bi-prediction, which stage bit 6 below computes).  Every vector used is the ME result of one of the CU's PU jobs, which
  * k_build_me_jobs' clip bounds relative to the CU origin, and every PU lies inside its CU, so the reads stay inside what
  * an_planes_cover (luma) and an_chroma_reach_ok (chroma) check; a value-32 run where either fails is refused too. */
 typedef struct {
@@ -698,6 +698,43 @@ typedef struct {
 /* the PART records of the CTU rows [ctuRow0, ctuRow1) into `out`, a full-frame host array of ncu records (synchronous);
  * refused before any value-32 run and for a bad row range */
 int x265cu_analyser_part_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x265cu_part_cu* out);
+
+/* ---------- inter estimate of every partition of a B slice's CUs ----------
+ * Stage bit 6 (value 64), PART_B: stage bit 5 for a B slice (x265cu_analyser_set_lists with numRefL1 > 0), i.e. checkInter_rd0_4
+ * (analysis.cpp:3023-3071) with predInterSearch's B-slice path (search.cpp:2473-2644) for every partition the geometry emits
+ * for every CU (8 to 64), in the same set and order as stage bit 5.  Per PU of the partition, on the analyser's cost model:
+ *   1. per list, the slot of lowest ME cost among the PU's jobs in that list (list 0 = slots [0, numRefL0)), ties to the
+ *      lowest slot; cost0 / cost1 are those jobs' ME costs (me_packed), mv0 / mv1 their vectors, mvp0 / mvp1 their MVPs;
+ *   2. the bi try, iff the partition is not 2Nx2N and the CU is not 8x8 (isBipredRestriction): bChromaSATD is chroma enabled,
+ *      subme > 2 and the PU's (pw/2) x (ph/2) chroma block has both sides a multiple of 4 (motion.cpp:212).  biCost = bufSATD of
+ *      the bi-prediction (addAvg of the two 14-bit predictions with bChromaSATD, else pixelavg_pp of the two pixel predictions),
+ *      + bufChromaSATD of the addAvg chroma with bChromaSATD, + mvcost(mv0 - mvp0) + mvcost(mv1 - mvp1).  The zero pair is
+ *      tried iff either vector is nonzero and both MVPs lie in the CU's setSearchRange(cu, 0, max(width, height)) (mvmax.y += 2,
+ *      both bounds << 2, as in BIDIR); its cost, the same formula at zero vectors, replaces biCost and the pair iff lower;
+ *   3. the PU is bi iff biCost < cost0 and biCost < cost1, else list 0 iff cost0 <= cost1, else list 1.
+ * The CU's prediction places each PU's final prediction: a uni PU's pixel prediction (as stage bit 5), a bi PU's addAvg of its
+ * two 14-bit predictions, luma and, with chroma enabled, Cb and Cr (predict.cpp:168-189), whichever path its biCost took.
+ * sa8d is the CU's sa8d over that prediction (+ Cb and Cr with chroma), cost = sa8d + every PU's mvcost: one vector for a uni
+ * PU, two for a bi PU.  As in BIDIR and PART there are no list-selection, reference-index or MVP-index bits, no checkBestMVP,
+ * no merge estimation of the rect / AMP PUs and no gating: the host adds its bits and decides.  Every PU keeps both lists'
+ * slot and vector, a uni PU too, so that the host can redo the decision with its own bits.
+ * One record per CU, read with x265cu_analyser_part_b_results; the records are allocated zeroed by the first value-64 run.
+ * Refused with -1 before any launch: value 64 on a P slice; any run of a B slice while a reference is weighted; a value-64 run
+ * where an_planes_cover or, with chroma, an_chroma_reach_ok fails (every vector read is a PU job's ME result or zero, inside
+ * the reach stage bit 5 checks). */
+typedef struct {
+    uint32_t cost[8], sa8d[8];     /* indexed by PartSize as x265cu_part_cu; UINT32_MAX where not evaluated */
+    uint32_t biCost[8][2];         /* per PU, after the zero try; UINT32_MAX where the bi try did not run or there is no PU */
+    int8_t   interDir[8][2];       /* 1 L0, 2 L1, 3 bi; 0 where there is no PU */
+    int8_t   ref[8][2][2];         /* [part][pu][list] slot of that list's best job; -1 where there is no PU */
+    uint8_t  zero[8][2];           /* 1: the zero pair replaced the searched pair */
+    int16_t  mv[8][2][2][2];       /* [part][pu][list] that list's vector (the bi pair after the zero try: both 0 where zero is
+                                      set, whatever interDir; the searched vector is then the slot's ME result); 0 where there is
+                                      no PU */
+} x265cu_part_b_cu;                /* 320 bytes */
+/* the PART_B records of the CTU rows [ctuRow0, ctuRow1) into `out`, a full-frame host array of ncu records (synchronous);
+ * refused before any value-64 run and for a bad row range */
+int x265cu_analyser_part_b_results(x265cu_analyser*, int ctuRow0, int ctuRow1, x265cu_part_b_cu* out);
 
 #ifdef __cplusplus
 }

@@ -69,8 +69,9 @@ struct x265cu_analyser
     // B slices (x265cu_analyser_set_lists): slots [0, numRefL0) are list 0, the rest list 1 (numRefL1 == 0: a P slice);
     // d_bidir = the BIDIR stage's record of every CU (stage bit 4), allocated by the first set_lists with a list 1
     int numRefL0, numRefL1; x265cu_bidir_cu* d_bidir;
-    // the PART stage's record of every CU (stage bit 5), allocated zeroed by the first run with that bit
-    x265cu_part_cu* d_part;
+    // the PART stage's record of every CU (stage bit 5), allocated zeroed by the first run with that bit; the same for the
+    // PART_B stage (stage bit 6)
+    x265cu_part_cu* d_part; x265cu_part_b_cu* d_partB;
 };
 
 static const int AN_MARGIN_X = 96, AN_MARGIN_Y = 80;       // picyuv.cpp:87-88 with maxCUSize 64
@@ -392,6 +393,14 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     else if ((stages & 32) && !an_planes_cover(a, r0, r1)) bad = "analyser: the reference planes do not cover what the PART stage can read";
     else if ((stages & 32) && a->chromaOn && (an_build_chroma_reach(a), !an_chroma_reach_ok(a, r0, r1)))
         bad = "analyser: the chroma planes do not cover what the PART stage's chroma MC can read";
+    // Reach of the PART_B stage: every vector it reads is a PU job's ME result, or zero in the bi try's zero pair, and every PU
+    // lies inside its CU, so its reads are those of the PART stage (above) or the CU's own blocks at zero, inside what the
+    // same two checks check.  Weighted slots never reach it: a B slice is refused while weighted (above).
+    else if ((stages & 64) && !a->numRefL1)
+        bad = "analyser: stage bit 6 (PART_B) needs a B slice (x265cu_analyser_set_lists with numRefL1 > 0); stage bit 5 is a P slice's";
+    else if ((stages & 64) && !an_planes_cover(a, r0, r1)) bad = "analyser: the reference planes do not cover what the PART_B stage can read";
+    else if ((stages & 64) && a->chromaOn && (an_build_chroma_reach(a), !an_chroma_reach_ok(a, r0, r1)))
+        bad = "analyser: the chroma planes do not cover what the PART_B stage's chroma MC can read";
     if (bad) { x265cu_set_error(bad, cudaErrorInvalidValue, __FILE__, __LINE__); return -1; }
     const int job0 = a->rowJob[r0], nj = a->rowJob[r1] - job0;
     const int cu0 = a->rowCu[r0], ncu = a->rowCu[r1] - cu0;
@@ -400,6 +409,11 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
     if ((stages & 32) && !a->d_part && !(a->d_part = (x265cu_part_cu*)an_alloc_zeroed(c, sizeof(x265cu_part_cu) * a->ncu)))
     {
         x265cu_set_error("analyser: no device memory for the PART records", cudaErrorMemoryAllocation, __FILE__, __LINE__);
+        return -1;
+    }
+    if ((stages & 64) && !a->d_partB && !(a->d_partB = (x265cu_part_b_cu*)an_alloc_zeroed(c, sizeof(x265cu_part_b_cu) * a->ncu)))
+    {
+        x265cu_set_error("analyser: no device memory for the PART_B records", cudaErrorMemoryAllocation, __FILE__, __LINE__);
         return -1;
     }
     a->ev_valid = stages;
@@ -459,7 +473,7 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
         if (depth == 8 ? launch_bidir<uint8_t>(c, b, lists, n) : launch_bidir<uint16_t>(c, b, lists, n)) return -1;
     }
-    if ((stages & 32) && ncu > 0)
+    if ((stages & 96) && ncu > 0)
     {
         PartArgs q;
         q.fenc[0] = a->d_fenc + a->orgBytes; q.refs[0] = a->d_refTable; q.stride = a->stride; q.chroma = a->chromaOn;
@@ -473,7 +487,14 @@ static int an_run(x265cu_analyser* a, int stages, int r0, int r1)
         q.out = a->d_part;
         const int32_t* lists[4]; int n[4];
         for (int k = 0; k < 4; k++) { lists[k] = a->d_cuBy[k] + a->rowCuBy[k][r0]; n[k] = a->rowCuBy[k][r1] - a->rowCuBy[k][r0]; }
-        if (depth == 8 ? launch_part<uint8_t>(c, q, lists, n) : launch_part<uint16_t>(c, q, lists, n)) return -1;
+        if ((stages & 32) && (depth == 8 ? launch_part<uint8_t>(c, q, lists, n) : launch_part<uint16_t>(c, q, lists, n))) return -1;
+        if (stages & 64)
+        {
+            PartBArgs b;
+            b.p = q; b.numRefL0 = a->numRefL0; b.width = a->p.width; b.height = a->p.height;
+            b.chromaSatd = a->chromaOn && a->p.subme > 2; b.out = a->d_partB;
+            if (depth == 8 ? launch_part_b<uint8_t>(c, b, lists, n) : launch_part_b<uint16_t>(c, b, lists, n)) return -1;
+        }
     }
     CU_CHECK(cudaEventRecord(a->ev[5], c->stream));
     if ((stages & 2) && ntu > 0 && an_residual(a, false, cu0, ncu, r0, r1)) return -1;
@@ -632,7 +653,7 @@ void x265cu_analyser_destroy(x265cu_analyser* a)
     cudaFree(a->d_reconCTable); cudaFree(a->d_cu_sseC); cudaFree(a->d_cu_numsigC);
     for (int r = 0; r < 16; r++) { cudaFree(a->d_wrefs[r]); cudaFree(a->d_wrefC[r][0]); cudaFree(a->d_wrefC[r][1]); }
     cudaFree(a->d_meRefTable); cudaFree(a->d_meCbTable); cudaFree(a->d_meCrTable); cudaFree(a->d_wtab); cudaFree(a->d_wjobs);
-    cudaFree(a->d_bidir); cudaFree(a->d_part);
+    cudaFree(a->d_bidir); cudaFree(a->d_part); cudaFree(a->d_partB);
     x265cu_host_free(a->h_fenc); x265cu_host_free(a->h_field);
     delete a;
 }
@@ -1069,6 +1090,22 @@ int x265cu_analyser_part_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, x
     cudaSetDevice(c->device);
     const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
     if (nc) CU_CHECK(cudaMemcpyAsync(out + c0, a->d_part + c0, sizeof(x265cu_part_cu) * nc, cudaMemcpyDeviceToHost, c->stream));
+    CU_CHECK(cudaStreamSynchronize(c->stream));
+    return 0;
+}
+
+// the PART_B records of the CTU rows [r0, r1) into a full-frame sized host array (synchronous)
+int x265cu_analyser_part_b_results(x265cu_analyser* a, int ctuRow0, int ctuRow1, x265cu_part_b_cu* out)
+{
+    if (!a->d_partB || ctuRow0 < 0 || ctuRow1 > a->ctuRows || ctuRow0 > ctuRow1)
+    {
+        x265cu_set_error("x265cu_analyser_part_b_results: no run with stage bit 6 (PART_B) yet, or a bad CTU row range", cudaErrorInvalidValue, __FILE__, __LINE__);
+        return -1;
+    }
+    x265cu_ctx* c = a->ctx;
+    cudaSetDevice(c->device);
+    const size_t c0 = a->rowCu[ctuRow0], nc = a->rowCu[ctuRow1] - c0;
+    if (nc) CU_CHECK(cudaMemcpyAsync(out + c0, a->d_partB + c0, sizeof(x265cu_part_b_cu) * nc, cudaMemcpyDeviceToHost, c->stream));
     CU_CHECK(cudaStreamSynchronize(c->stream));
     return 0;
 }

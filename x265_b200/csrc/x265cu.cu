@@ -411,6 +411,10 @@ static_assert(sizeof(x265cu_wp_frame) == 112 && sizeof(x265cu_wp_params) == 28 &
 static_assert(sizeof(x265cu_deblock_unit) == 16 && sizeof(x265cu_deblock_params) == 24, "deblocking records (include/x265_b200.h)");
 static_assert(sizeof(x265cu_bidir_cu) == 20, "BIDIR record (include/x265_b200.h)");
 static_assert(sizeof(x265cu_part_cu) == 144, "PART record (include/x265_b200.h)");
+static_assert(sizeof(x265cu_part_b_cu) == 320, "PART_B record (include/x265_b200.h)");
+static_assert(offsetof(x265cu_part_b_cu, biCost) == 64 && offsetof(x265cu_part_b_cu, interDir) == 128 &&
+              offsetof(x265cu_part_b_cu, ref) == 144 && offsetof(x265cu_part_b_cu, zero) == 176 && offsetof(x265cu_part_b_cu, mv) == 192,
+              "PART_B record layout (include/x265_b200.h, tests/test_gpu_x_partitions_b.py)");
 
 // the argument rules of the deblocking calls on one set of planes; NULL when they hold
 static const char* deblock_check(const char* fn, int depth, int width, int height, const void* luma, const void* cb,

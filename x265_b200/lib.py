@@ -395,6 +395,11 @@ _AN_PROTOS["x265cu_analyser_part_results"] = (I, [P, I, I, P])
 # x265cu_part_cu (include/x265_b200.h): entries indexed by PartSize (2Nx2N 0, 2NxN 1, Nx2N 2, NxN 3, 2NxnU 4, 2NxnD 5,
 # nLx2N 6, nRx2N 7)
 PART_CU = np.dtype([("cost", np.uint32, 8), ("sa8d", np.uint32, 8), ("ref", np.int8, (8, 2)), ("mv", np.int16, (8, 2, 2))])
+STAGE_PART_B = 64                         # analyser stage bit 6: the inter estimate of every partition of a B slice's CUs
+_AN_PROTOS["x265cu_analyser_part_b_results"] = (I, [P, I, I, P])
+# x265cu_part_b_cu (include/x265_b200.h): entries indexed by PartSize as PART_CU; per PU [pu], per list [pu][list]
+PART_B_CU = np.dtype([("cost", np.uint32, 8), ("sa8d", np.uint32, 8), ("biCost", np.uint32, (8, 2)), ("interDir", np.int8, (8, 2)),
+                      ("ref", np.int8, (8, 2, 2)), ("zero", np.uint8, (8, 2)), ("mv", np.int16, (8, 2, 2, 2))])
 _AN_PROTOS["x265cu_propagate_cost_batch"] = (I, [P, P, P, P, P, P, C.c_double, I64])
 _AN_PROTOS["x265cu_lowres_intra_batch"] = (I, [P, I, P, I, I, I, I, I])
 _AN_PROTOS["x265cu_lookahead_cost_batch"] = (I, [P, I, P, I, I, I, I, P])
@@ -608,6 +613,16 @@ class Analyser:
         out = np.zeros(self.ncu, PART_CU) if out is None else out
         assert out.shape == (self.ncu,) and out.dtype == PART_CU
         self.lib.check(self.lib.L.x265cu_analyser_part_results(self.h, r0, r1, out.ctypes.data))
+        return out
+
+    # ---- the inter estimate of every partition of a B slice's CUs (stage bit 6) ----
+    def part_b_results(self, r0=0, r1=None, out=None):
+        """The PART_B record (PART_B_CU) of every CU of the CTU rows [r0, r1) (default: all) into the given full-frame array or
+        a new zeroed one; returns it.  Needs a run with stage bit 6 (STAGE_PART_B) first."""
+        r1 = self.ctu_rows if r1 is None else r1
+        out = np.zeros(self.ncu, PART_B_CU) if out is None else out
+        assert out.shape == (self.ncu,) and out.dtype == PART_B_CU
+        self.lib.check(self.lib.L.x265cu_analyser_part_b_results(self.h, r0, r1, out.ctypes.data))
         return out
 
     def chroma_plane_shape(self):
