@@ -91,6 +91,9 @@ void orc_interp_hvpp(const pixel* s, intptr_t ss, pixel* d, intptr_t ds, int idx
 /* ---- prediction costs around the motion search (oracle_pred.c: search.cpp:1901-2023, 2474-2607; predict.cpp:76-420) ---- */
 struct orc_pred_job_s;
 int orc_pred_cost(const struct orc_pred_job_s* j);      /* the job struct is defined in oracle_pred.c / tests/pred_helpers.py */
+/* orc_pred_cost over x265cu_pred_job records, planes and tables as x265ref_pred_cost_batch (oracle/ref_shim.cpp) takes them */
+int orc_pred_cost_batch(const pixel* fenc, const pixel* fencCb, const pixel* fencCr, const pixel* const* refs, const pixel* const* refCb,
+                        const pixel* const* refCr, intptr_t stride, intptr_t cstride, const void* jobs, int n, int32_t* out);
 
 /* ---- transforms / quant (dct.cpp:43-742) ---- */
 const int16_t* orc_dct_matrix(int n);        /* n x n HEVC matrix, regenerated from the 32-pt basis */

@@ -126,3 +126,40 @@ int orc_pred_cost(const orc_pred_job* j)
         for (int p = 0; p < 2; p++) cost += orc_satd(predC[p], 32, j->fenc[1 + p], j->cstride, cw, ch);
     return cost;
 }
+
+/* orc_pred_cost over a job list in the batched entry point's layout (include/x265_b200.h: x265cu_pred_job), with the planes
+ * and tables of x265ref_pred_cost_batch (oracle/ref_shim.cpp): planes at the picture origin, refs / refCb / refCr indexed by
+ * ref0 / ref1, the chroma origin of the luma offset at ((offset / stride) >> 1) * cstride + ((offset % stride) >> 1).
+ * fencCb == NULL: no chroma planes, so no job gets the chroma term (as x265cu_pred_cost_batch with chroma == NULL). */
+typedef struct { int32_t offset; int16_t pw, ph; int8_t ref0, ref1; uint8_t cost, flags; int16_t mv0[2], mv1[2]; } orc_pred_batch_job;
+
+int orc_pred_cost_batch(const pixel* fenc, const pixel* fencCb, const pixel* fencCr, const pixel* const* refs, const pixel* const* refCb,
+                        const pixel* const* refCr, intptr_t stride, intptr_t cstride, const void* jobsv, int n, int32_t* out)
+{
+    const orc_pred_batch_job* jobs = (const orc_pred_batch_job*)jobsv;
+    for (int i = 0; i < n; i++)
+    {
+        const orc_pred_batch_job* b = &jobs[i];
+        const intptr_t coff = ((b->offset / stride) >> 1) * cstride + ((b->offset % stride) >> 1);
+        const int chroma = (b->flags & 1) && fencCb;
+        orc_pred_job j;
+        memset(&j, 0, sizeof(j));
+        j.fenc[0] = fenc + b->offset;
+        if (chroma) { j.fenc[1] = fencCb + coff; j.fenc[2] = fencCr + coff; }
+        if (b->ref0 >= 0)
+        {
+            j.ref0[0] = refs[b->ref0] + b->offset;
+            if (chroma) { j.ref0[1] = refCb[b->ref0] + coff; j.ref0[2] = refCr[b->ref0] + coff; }
+        }
+        if (b->ref1 >= 0)
+        {
+            j.ref1[0] = refs[b->ref1] + b->offset;
+            if (chroma) { j.ref1[1] = refCb[b->ref1] + coff; j.ref1[2] = refCr[b->ref1] + coff; }
+        }
+        j.stride = stride; j.cstride = cstride; j.w = b->pw; j.h = b->ph;
+        j.mv0[0] = b->mv0[0]; j.mv0[1] = b->mv0[1]; j.mv1[0] = b->mv1[0]; j.mv1[1] = b->mv1[1];
+        j.cost = b->cost; j.chroma = chroma; j.biAvgPP = (b->flags >> 1) & 1;
+        out[i] = orc_pred_cost(&j);
+    }
+    return 0;
+}
